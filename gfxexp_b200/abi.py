@@ -275,7 +275,8 @@ NRC_TRAIN_BUFFER_SIZE = 2 * 65536   # shared::trainBufferSize (neural_radiance_c
 NRC_TRAINING_DATA_PER_FRAME = 65536
 NRC_INVALID_VERTEX = 0x007FFFFF     # shared::invalidVertexDataIndex
 (NRC_STATE_NUM_TRAINING_DATA, NRC_STATE_TILE_SIZE, NRC_STATE_OFFSET_UNBIASED_TILE, NRC_STATE_OFFSET_TRAINING_PATH,
- NRC_STATE_TARGET_MIN, NRC_STATE_TARGET_MAX, NRC_STATE_TARGET_AVG, NRC_STATE_NUM_INFERENCE_QUERIES) = 0, 2, 6, 7, 8, 11, 20, 26
+ NRC_STATE_TARGET_MIN, NRC_STATE_TARGET_MAX, NRC_STATE_TARGET_AVG, NRC_STATE_NUM_INFERENCE_QUERIES,
+ NRC_STATE_NUM_SUFFIX_QUERIES) = 0, 2, 6, 7, 8, 11, 20, 26, 27
 
 
 def nrc_num_suffixes(width: int, height: int) -> int:

@@ -1299,9 +1299,49 @@ static void tcnnInitialParams(uint32_t seed, uint32_t numHiddenLayers, uint32_t 
         }
 }
 
+// Dynamic shared memory of the kernels whose footprint grows with the depth: the launches request these sizes, and
+// gfx_nrc_create rejects a depth for which one of them exceeds the device's per-block limit.
+constexpr uint32_t kMaxTcTrainHiddenLayers = 3; // deeper networks train on k_nrcTrain
+static size_t nrcInferFusedSmem(uint32_t numMatrixWeights) { return kATileBytes + (size_t)numMatrixWeights * 2; }
+static size_t nrcInferMlpSmem(uint32_t numMatrixWeights) {
+    return kATileBytes + 2 * sizeof(NrcTileStage) + 128 * kOutputDims * 4 + (size_t)numMatrixWeights * 2;
+}
+static size_t nrcTrainTcSmem(uint32_t numMatrixWeights, uint32_t numHiddenLayers) {
+    return (size_t)numMatrixWeights * 4 + (size_t)(numHiddenLayers + 1) * kATileBytes + 3 * (size_t)kATileBytes;
+}
+static size_t nrcTrainSmem(uint32_t numMatrixWeights, uint32_t numHiddenLayers) {
+    return ((size_t)numMatrixWeights + (size_t)(numHiddenLayers + 2) * 128 * kRowStride) * 2;
+}
+
 } // namespace gfx
 
 using namespace gfx;
+
+// every kernel that can train or infer a network of this depth fits in one block's shared memory (dynamic + static)
+static int nrcCheckSharedMemory(gfx_ctx* ctx, const gfx_nrc* n) {
+    int limit = 0;
+    GFX_CUDA(ctx, cudaDeviceGetAttribute(&limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+    const uint32_t M = n->numMatrixWeights, H = n->numHiddenLayers;
+    const struct { const void* kernel; const char* name; size_t dynamicBytes; } kernels[] = {
+        { (const void*)k_nrcInfer, "k_nrcInfer", nrcInferFusedSmem(M) },
+        { (const void*)k_nrcInferMlp, "k_nrcInferMlp", nrcInferMlpSmem(M) },
+        { (const void*)k_nrcTrainTc, "k_nrcTrainTc", H <= kMaxTcTrainHiddenLayers ? nrcTrainTcSmem(M, H) : 0 },
+        { (const void*)k_nrcTrain, "k_nrcTrain", nrcTrainSmem(M, H) },
+    };
+    for (const auto &k : kernels) {
+        cudaFuncAttributes attr;
+        GFX_CUDA(ctx, cudaFuncGetAttributes(&attr, k.kernel));
+        const size_t need = k.dynamicBytes + attr.sharedSizeBytes;
+        if (need > (size_t)limit) {
+            char msg[256];
+            snprintf(msg, sizeof(msg), "gfx_nrc_create: %u hidden layers need %zu bytes of shared memory per block in %s, "
+                     "more than the device's limit of %d bytes", H, need, k.name, limit);
+            ctx->setError(msg);
+            return GFX_ERR_UNSUPPORTED;
+        }
+    }
+    return GFX_OK;
+}
 
 #define NRC_CUDA(nrc, call) GFX_CUDA((nrc)->ctx, call)
 
@@ -1325,6 +1365,11 @@ int gfx_nrc_create(gfx_ctx* ctx, uint32_t numHiddenLayers, float learningRate, g
     n->numHiddenLayers = numHiddenLayers;
     n->learningRate = learningRate;
     setupLevels(n);
+    const int fits = nrcCheckSharedMemory(ctx, n);
+    if (fits != GFX_OK) {
+        delete n;
+        return fits;
+    }
     const size_t P = n->numParams;
     GFX_CUDA(ctx, cudaMalloc(&n->params, P * 2));
     GFX_CUDA(ctx, cudaMalloc(&n->paramsEma, P * 2));
@@ -1489,7 +1534,7 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
     const char* fusedEnv = getenv("GFX_NRC_INFER_FUSED");
     const bool aligned = (reinterpret_cast<uintptr_t>(inputData) & 15u) == 0 && (reinterpret_cast<uintptr_t>(predictionData) & 15u) == 0;
     if ((fusedEnv && fusedEnv[0] == '1') || !aligned) {
-        const size_t smem = kATileBytes + (size_t)n->numMatrixWeights * 2;
+        const size_t smem = nrcInferFusedSmem(n->numMatrixWeights);
         NRC_CUDA(n, cudaFuncSetAttribute(k_nrcInfer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         const uint32_t grid = numTiles < (uint32_t)sms * 6 ? numTiles : (uint32_t)sms * 6;
         GFX_TIMED(n->ctx, s, "nrc_infer");
@@ -1505,7 +1550,7 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
     rc = nrcGridEncodeLaunch(n, s, inputData, numData, numDataPtr, true);
     if (rc != GFX_OK)
         return rc;
-    const size_t smem = kATileBytes + 2 * sizeof(NrcTileStage) + 128 * kOutputDims * 4 + (size_t)n->numMatrixWeights * 2;
+    const size_t smem = nrcInferMlpSmem(n->numMatrixWeights);
     NRC_CUDA(n, cudaFuncSetAttribute(k_nrcInferMlp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const uint32_t ctasPerSm = (uint32_t)(220 * 1024 / (smem + 1024));
     const uint32_t maxGrid = (uint32_t)sms * (ctasPerSm ? ctasPerSm : 1u);
@@ -1627,8 +1672,8 @@ int gfx_nrc_train(gfx_nrc* n, void* stream, const float* inputData, const float*
     // networks whose activation tiles do not fit in shared memory and as the A/B switch GFX_NRC_TRAIN_CUDACORES=1.
     const char* cudaCoresEnv = getenv("GFX_NRC_TRAIN_CUDACORES");
     const bool forceCudaCores = cudaCoresEnv && cudaCoresEnv[0] == '1';
-    if (n->numHiddenLayers <= 3 && !forceCudaCores) {
-        const size_t smem = (size_t)n->numMatrixWeights * 4 + (size_t)(n->numHiddenLayers + 1) * kATileBytes + 3 * (size_t)kATileBytes;
+    if (n->numHiddenLayers <= kMaxTcTrainHiddenLayers && !forceCudaCores) {
+        const size_t smem = nrcTrainTcSmem(n->numMatrixWeights, n->numHiddenLayers);
         NRC_CUDA(n, cudaFuncSetAttribute(k_nrcTrainTc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         { GFX_TIMED(n->ctx, s, "nrc_train_prep_weights");
         k_nrcPrepTrainWeights<<<32, 256, 0, s>>>(n->params, n->numHiddenLayers, reinterpret_cast<__half*>(n->trainBlobFwd),
@@ -1640,7 +1685,7 @@ int gfx_nrc_train(gfx_nrc* n, void* stream, const float* inputData, const float*
                                                       n->loss); }
     }
     else {
-        const size_t smem = ((size_t)n->numMatrixWeights + (size_t)(n->numHiddenLayers + 2) * 128 * kRowStride) * 2;
+        const size_t smem = nrcTrainSmem(n->numMatrixWeights, n->numHiddenLayers);
         NRC_CUDA(n, cudaFuncSetAttribute(k_nrcTrain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         { GFX_TIMED(n->ctx, s, "nrc_train_fwd_bwd");
         k_nrcTrain<<<numData / 128, 128, smem, s>>>(n->levels, n->params, n->numMatrixWeights, n->numHiddenLayers, inputData,

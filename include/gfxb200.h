@@ -517,6 +517,11 @@ int gfx_regir_update_access(gfx_ctx* ctx, void* stream, const GfxFrameParams* pa
 
 /* ---- NRC network (network_interface.h:14-28) ------------------------------------------ */
 typedef struct gfx_nrc gfx_nrc;
+/* numHiddenLayers: 1..8 (GFX_ERR_INVALID_ARGUMENT otherwise), and only depths whose training and inference kernels fit in
+ * the device's shared memory per block (cudaDevAttrMaxSharedMemoryPerBlockOptin); a deeper network is rejected with
+ * GFX_ERR_UNSUPPORTED and an error string that names the kernel, its need and the limit.  On an H100 (232 448 bytes)
+ * that is 1..7: at 8 the CUDA-core training kernel (the only one for more than 3 hidden layers) needs 236 544 bytes of
+ * dynamic shared memory alone. */
 int gfx_nrc_create(gfx_ctx* ctx, uint32_t numHiddenLayers, float learningRate, gfx_nrc** out);
 void gfx_nrc_destroy(gfx_nrc* nrc);
 /* inputData: device float[14, numData] (column per query), predictionData: device float[3, numData];

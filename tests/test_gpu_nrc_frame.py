@@ -125,6 +125,58 @@ def test_nrc_frames_bit_exact(gfx_ctx, oracle, max_path_length, scene_name):
     net.close()
 
 
+@pytest.mark.parametrize("w,h,strips", [(192, 108, [(0, 34), (34, 80), (80, 108)]),
+                                         (1920, 1080, [(0, 360), (360, 1001), (1001, 1080)])])
+def test_frame_inference_matches_direct_inference(gfx_ctx, w, h, strips):
+    """gfx_nrc_frame_infer infers as many queries as the device-side count in the state block says (pixels + training-suffix
+    slots, padded to the 128-query tile) and leaves the rows beyond it alone; its predictions are the bits gfx_nrc_infer gives
+    the same queries in launches of one tile per CTA.  gfx_nrc_frame_infer_rows (one strip of rows of a frame split across GPUs)
+    gives the same bits on the strip's pixel rows and on every suffix query, and writes nothing else."""
+    import torch
+    scene = scenes.small_city_scene()
+    gfx_ctx.upload_scene(scene)
+    gfx_ctx.build_bvh()
+    gfx_ctx.create_frame(w, h)
+    gfx_ctx.build_light_distributions(0)
+    net = engine.NeuralRadianceCache(gfx_ctx, 2, 1e-2)
+    net.set_params(engine.random_nrc_params(net.num_params, 64 * 64 * 2 + 16 * 64, seed=19, grid_amplitude=0.1))
+    p = abi.default_frame_params(scene, w, h)
+    gfx_ctx.gbuffer(p)
+    gfx_ctx.nrc_preprocess(p, 0x2545F491, 0x9E3779B9, True)
+    gfx_ctx.pathtrace(p, abi.PT_NRC)
+    n, capacity = w * h, abi.nrc_query_capacity(w, h)
+    sentinel = np.full((capacity, 3), 0x7FC0DEAD, dtype=np.uint32).view(np.float32)  # a NaN no kernel produces
+
+    gfx_ctx.upload(abi.BUF_NRC_INFERRED_RADIANCE, 0, sentinel)
+    gfx_ctx.nrc_frame_infer(net)
+    frame = gfx_ctx.download_linear(abi.BUF_NRC_INFERRED_RADIANCE)
+    st = gfx_ctx.download_linear(abi.BUF_NRC_STATE)[:, 0]
+    count, num_suffix = int(st[abi.NRC_STATE_NUM_INFERENCE_QUERIES]), int(st[abi.NRC_STATE_NUM_SUFFIX_QUERIES])
+    assert count % 128 == 0 and n < count <= capacity and count == n + num_suffix, (count, num_suffix, capacity)
+    _same(frame[count:], sentinel[count:], "rows beyond the device-side query count")
+
+    queries = torch.from_numpy(gfx_ctx.download_linear(abi.BUF_NRC_INFERENCE_QUERY)[:count]).cuda()
+    direct = torch.empty((count, 3), device="cuda")
+    step = torch.cuda.get_device_properties(0).multi_processor_count * 128
+    for lo in range(0, count, step):
+        m = min(step, count - lo)
+        net.infer(queries[lo:lo + m], direct[lo:lo + m], m)
+    torch.cuda.synchronize()
+    _same(frame[:count], direct.cpu().numpy(), "frame inference vs gfx_nrc_infer in single-wave launches")
+
+    for lo, hi in strips:
+        gfx_ctx.upload(abi.BUF_NRC_INFERRED_RADIANCE, 0, sentinel)
+        gfx_ctx._check(gfx_ctx.lib.gfx_nrc_frame_infer_rows(gfx_ctx.h, net.h, None, lo, hi), "gfx_nrc_frame_infer_rows")
+        got = gfx_ctx.download_linear(abi.BUF_NRC_INFERRED_RADIANCE)
+        first, end = lo * w, lo * w + ((hi - lo) * w + 127) // 128 * 128  # the strip's pixels, padded to whole tiles
+        _same(got[first:hi * w], frame[first:hi * w], f"rows {lo}..{hi}: pixel queries")
+        _same(got[n:n + num_suffix], frame[n:n + num_suffix], f"rows {lo}..{hi}: suffix queries")
+        _same(got[:first], sentinel[:first], f"rows {lo}..{hi}: pixels before the strip")
+        _same(got[end:n], sentinel[end:n], f"rows {lo}..{hi}: pixels after the strip")
+        _same(got[n + num_suffix:], sentinel[n + num_suffix:], f"rows {lo}..{hi}: beyond the suffix queries")
+    net.close()
+
+
 def test_nrc_frame_wrapper_and_tile_controller(gfx_ctx):
     """the one-call frame (no host read-backs) keeps the training-record count near 65 536 * (tile area ratio)
     and produces a finite image"""
