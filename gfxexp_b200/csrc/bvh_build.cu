@@ -10,11 +10,15 @@
 //   1 flatten      : world-space TriangleStorage per (instance, mesh, prim) + AABB + scene bounds
 //   2 morton       : 63-bit Morton key of the AABB centre
 //   3 sort         : cub::DeviceRadixSort (key, triangle id)
-//   4 hierarchy    : default: PLOC (Meister & Bittner 2018) - parallel locally-ordered agglomerative clustering of the
-//                    Morton-ordered leaves (each cluster merges with its mutual nearest neighbour, by surface area of
-//                    the union, within +-16 positions; compaction; repeat) = a SAH-quality binary tree;
-//                    GFX_BVH_BUILD_FAST: Karras 2012 binary radix tree over the sorted keys + bottom-up refit with
-//                    per-node arrival counters (a faster build, ~40 % more node visits per ray)
+//   4 hierarchy    : default: binned SAH, top-down and level-synchronous (16 bins per axis, stable partition of the
+//                    Morton-ordered slice; nodes above kSahHugeNode triangles are split by many blocks);
+//                    GFX_BVH_BUILD_PLOC: PLOC (Meister & Bittner 2018) - parallel locally-ordered agglomerative clustering
+//                    of the Morton-ordered leaves (each cluster merges with its mutual nearest neighbour, by surface area
+//                    of the union, within +-16 positions; compaction; repeat);
+//                    GFX_BVH_BUILD_FAST (and any scene of fewer than 3 triangles): Karras 2012 binary radix tree over the
+//                    sorted keys + bottom-up refit with per-node arrival counters (the fastest build, more node visits per ray)
+//   The SAH and LBVH trees are deterministic functions of the triangles; oracle/gpu_bvh.cpp restates both, and the tests
+//   compare the exported trees with it node by node.
 //   5 collapse     : level-synchronous top-down collapse of the binary tree into 8-wide nodes
 //                    (largest-surface-area child is opened first, like the reference's task loop
 //                    :777-800), leaves of <= maxLeaf triangles (default 2), conservative 8-bit quantisation.
@@ -34,6 +38,13 @@ __device__ __forceinline__ uint32_t orderedFromFloat(float f) {
 __device__ __forceinline__ float floatFromOrdered(uint32_t u) {
     return __uint_as_float(u ^ (u >= 0x80000000u ? 0x80000000u : 0xFFFFFFFFu));
 }
+// Every box bound of the builders is a minimum / maximum in the order of these integer images, in which -0 < +0.  fminf /
+// fmaxf leave the sign of a zero result unspecified when the inputs are zeros of both signs, so a bound reduced with them
+// could depend on the reduction order (and differ between the huge, big and small SAH kernels); with the images it cannot.
+__device__ __forceinline__ float minOrdered(float a, float b) { return orderedFromFloat(b) < orderedFromFloat(a) ? b : a; }
+__device__ __forceinline__ float maxOrdered(float a, float b) { return orderedFromFloat(b) > orderedFromFloat(a) ? b : a; }
+__device__ __forceinline__ f3 minOrdered(const f3 &a, const f3 &b) { return f3(minOrdered(a.x, b.x), minOrdered(a.y, b.y), minOrdered(a.z, b.z)); }
+__device__ __forceinline__ f3 maxOrdered(const f3 &a, const f3 &b) { return f3(maxOrdered(a.x, b.x), maxOrdered(a.y, b.y), maxOrdered(a.z, b.z)); }
 
 // ---- 1. flatten -----------------------------------------------------------------------------
 __global__ void k_flatten(DevScene scene, const uint32_t* __restrict__ geomTriOffsets, uint32_t numGeoms,
@@ -64,21 +75,21 @@ __global__ void k_flatten(DevScene scene, const uint32_t* __restrict__ geomTriOf
         tris[3 * (size_t)t + 0] = make_float4(pA.x, pA.y, pA.z, pB.x);
         tris[3 * (size_t)t + 1] = make_float4(pB.y, pB.z, pC.x, pC.y);
         tris[3 * (size_t)t + 2] = make_float4(pC.z, __uint_as_float(g), __uint_as_float(prim), 0.0f);
-        lo = min3(min3(pA, pB), pC);
-        hi = max3(max3(pA, pB), pC);
+        lo = minOrdered(minOrdered(pA, pB), pC);
+        hi = maxOrdered(maxOrdered(pA, pB), pC);
         triLo[t] = make_float4(lo.x, lo.y, lo.z, 0.0f);
         triHi[t] = make_float4(hi.x, hi.y, hi.z, 0.0f);
     }
-    // block reduction of the scene bounds, then 6 atomics per block
-    typedef cub::BlockReduce<float, 256> BR;
+    // block reduction of the scene bounds (ordered images), then 6 atomics per block
+    typedef cub::BlockReduce<uint32_t, 256> BR;
     __shared__ typename BR::TempStorage tmp;
-    float v;
-    v = BR(tmp).Reduce(lo.x, cub::Min()); __syncthreads(); if (threadIdx.x == 0) atomicMin(sceneBounds + 0, orderedFromFloat(v));
-    v = BR(tmp).Reduce(lo.y, cub::Min()); __syncthreads(); if (threadIdx.x == 0) atomicMin(sceneBounds + 1, orderedFromFloat(v));
-    v = BR(tmp).Reduce(lo.z, cub::Min()); __syncthreads(); if (threadIdx.x == 0) atomicMin(sceneBounds + 2, orderedFromFloat(v));
-    v = BR(tmp).Reduce(hi.x, cub::Max()); __syncthreads(); if (threadIdx.x == 0) atomicMax(sceneBounds + 3, orderedFromFloat(v));
-    v = BR(tmp).Reduce(hi.y, cub::Max()); __syncthreads(); if (threadIdx.x == 0) atomicMax(sceneBounds + 4, orderedFromFloat(v));
-    v = BR(tmp).Reduce(hi.z, cub::Max()); __syncthreads(); if (threadIdx.x == 0) atomicMax(sceneBounds + 5, orderedFromFloat(v));
+    uint32_t v;
+    v = BR(tmp).Reduce(orderedFromFloat(lo.x), cub::Min()); __syncthreads(); if (threadIdx.x == 0) atomicMin(sceneBounds + 0, v);
+    v = BR(tmp).Reduce(orderedFromFloat(lo.y), cub::Min()); __syncthreads(); if (threadIdx.x == 0) atomicMin(sceneBounds + 1, v);
+    v = BR(tmp).Reduce(orderedFromFloat(lo.z), cub::Min()); __syncthreads(); if (threadIdx.x == 0) atomicMin(sceneBounds + 2, v);
+    v = BR(tmp).Reduce(orderedFromFloat(hi.x), cub::Max()); __syncthreads(); if (threadIdx.x == 0) atomicMax(sceneBounds + 3, v);
+    v = BR(tmp).Reduce(orderedFromFloat(hi.y), cub::Max()); __syncthreads(); if (threadIdx.x == 0) atomicMax(sceneBounds + 4, v);
+    v = BR(tmp).Reduce(orderedFromFloat(hi.z), cub::Max()); __syncthreads(); if (threadIdx.x == 0) atomicMax(sceneBounds + 5, v);
 }
 
 // ---- 2. morton ------------------------------------------------------------------------------
@@ -188,8 +199,8 @@ __global__ void k_refit(int n, const uint32_t* __restrict__ sortedIds, const flo
         const volatile float4* vhi = boxHi;
         const float4 a = make_float4(vlo[li].x, vlo[li].y, vlo[li].z, 0), b = make_float4(vlo[ri].x, vlo[ri].y, vlo[ri].z, 0);
         const float4 c = make_float4(vhi[li].x, vhi[li].y, vhi[li].z, 0), d = make_float4(vhi[ri].x, vhi[ri].y, vhi[ri].z, 0);
-        boxLo[p] = make_float4(fminf(a.x, b.x), fminf(a.y, b.y), fminf(a.z, b.z), 0.0f);
-        boxHi[p] = make_float4(fmaxf(c.x, d.x), fmaxf(c.y, d.y), fmaxf(c.z, d.z), 0.0f);
+        boxLo[p] = make_float4(minOrdered(a.x, b.x), minOrdered(a.y, b.y), minOrdered(a.z, b.z), 0.0f);
+        boxHi[p] = make_float4(maxOrdered(c.x, d.x), maxOrdered(c.y, d.y), maxOrdered(c.z, d.z), 0.0f);
         __threadfence();
         p = parentOfInternal[p];
     }
@@ -558,34 +569,34 @@ __global__ void __launch_bounds__(BLOCK) k_sahSplit(SahArgs a) {
         (&sBinCount[0][0][0])[i] = 0u;
     __syncthreads();
 
-    // 1. bounds
+    // 1. bounds (ordered images throughout, so the result does not depend on which thread reduces which triangle)
     {
-        float lo[3] = { INFINITY, INFINITY, INFINITY }, hi[3] = { -INFINITY, -INFINITY, -INFINITY };
-        float clo[3] = { INFINITY, INFINITY, INFINITY }, chi[3] = { -INFINITY, -INFINITY, -INFINITY };
+        uint32_t lo[3] = { 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu }, hi[3] = { 0u, 0u, 0u };
+        uint32_t clo[3] = { 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu }, chi[3] = { 0u, 0u, 0u };
         for (uint32_t i = start + tid; i < end; i += BLOCK) {
             const uint32_t t = a.order[i];
             const float4 l = a.triLo[t], h = a.triHi[t];
             const float bl[3] = { l.x, l.y, l.z }, bh[3] = { h.x, h.y, h.z };
 #pragma unroll
             for (int d = 0; d < 3; ++d) {
-                const float c = 0.5f * bl[d] + 0.5f * bh[d];
-                lo[d] = fminf(lo[d], bl[d]); hi[d] = fmaxf(hi[d], bh[d]);
-                clo[d] = fminf(clo[d], c); chi[d] = fmaxf(chi[d], c);
+                const uint32_t c = orderedFromFloat(0.5f * bl[d] + 0.5f * bh[d]);
+                lo[d] = min(lo[d], orderedFromFloat(bl[d])); hi[d] = max(hi[d], orderedFromFloat(bh[d]));
+                clo[d] = min(clo[d], c); chi[d] = max(chi[d], c);
             }
         }
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
             for (int off = 16; off > 0; off >>= 1) {
-                lo[d] = fminf(lo[d], __shfl_xor_sync(0xFFFFFFFFu, lo[d], off));
-                hi[d] = fmaxf(hi[d], __shfl_xor_sync(0xFFFFFFFFu, hi[d], off));
-                clo[d] = fminf(clo[d], __shfl_xor_sync(0xFFFFFFFFu, clo[d], off));
-                chi[d] = fmaxf(chi[d], __shfl_xor_sync(0xFFFFFFFFu, chi[d], off));
+                lo[d] = min(lo[d], __shfl_xor_sync(0xFFFFFFFFu, lo[d], off));
+                hi[d] = max(hi[d], __shfl_xor_sync(0xFFFFFFFFu, hi[d], off));
+                clo[d] = min(clo[d], __shfl_xor_sync(0xFFFFFFFFu, clo[d], off));
+                chi[d] = max(chi[d], __shfl_xor_sync(0xFFFFFFFFu, chi[d], off));
             }
             if (lane == 0) {
-                atomicMin(&sBoundsLo[0][d], orderedFromFloat(lo[d]));
-                atomicMax(&sBoundsHi[0][d], orderedFromFloat(hi[d]));
-                atomicMin(&sBoundsLo[1][d], orderedFromFloat(clo[d]));
-                atomicMax(&sBoundsHi[1][d], orderedFromFloat(chi[d]));
+                atomicMin(&sBoundsLo[0][d], lo[d]);
+                atomicMax(&sBoundsHi[0][d], hi[d]);
+                atomicMin(&sBoundsLo[1][d], clo[d]);
+                atomicMax(&sBoundsHi[1][d], chi[d]);
             }
         }
     }
@@ -811,33 +822,33 @@ __global__ void __launch_bounds__(1024) k_sahHugeBounds(SahHugeArgs h) {
     uint32_t entry, begin, end;
     if (!sahHugeLocate(h.a, blockIdx.x, &entry, &begin, &end))
         return;
-    float lo[3] = { INFINITY, INFINITY, INFINITY }, hi[3] = { -INFINITY, -INFINITY, -INFINITY };
-    float clo[3] = { INFINITY, INFINITY, INFINITY }, chi[3] = { -INFINITY, -INFINITY, -INFINITY };
+    uint32_t lo[3] = { 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu }, hi[3] = { 0u, 0u, 0u };
+    uint32_t clo[3] = { 0xFFFFFFFFu, 0xFFFFFFFFu, 0xFFFFFFFFu }, chi[3] = { 0u, 0u, 0u };
     for (uint32_t i = begin + threadIdx.x; i < end; i += blockDim.x) {
         const uint32_t t = h.a.order[i];
         const float4 l = h.a.triLo[t], u = h.a.triHi[t];
         const float bl[3] = { l.x, l.y, l.z }, bh[3] = { u.x, u.y, u.z };
 #pragma unroll
         for (int d = 0; d < 3; ++d) {
-            const float c = 0.5f * bl[d] + 0.5f * bh[d];
-            lo[d] = fminf(lo[d], bl[d]); hi[d] = fmaxf(hi[d], bh[d]);
-            clo[d] = fminf(clo[d], c); chi[d] = fmaxf(chi[d], c);
+            const uint32_t c = orderedFromFloat(0.5f * bl[d] + 0.5f * bh[d]);
+            lo[d] = min(lo[d], orderedFromFloat(bl[d])); hi[d] = max(hi[d], orderedFromFloat(bh[d]));
+            clo[d] = min(clo[d], c); chi[d] = max(chi[d], c);
         }
     }
     SahHugeNode &N = h.nodes[entry];
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
         for (int off = 16; off > 0; off >>= 1) {
-            lo[d] = fminf(lo[d], __shfl_xor_sync(0xFFFFFFFFu, lo[d], off));
-            hi[d] = fmaxf(hi[d], __shfl_xor_sync(0xFFFFFFFFu, hi[d], off));
-            clo[d] = fminf(clo[d], __shfl_xor_sync(0xFFFFFFFFu, clo[d], off));
-            chi[d] = fmaxf(chi[d], __shfl_xor_sync(0xFFFFFFFFu, chi[d], off));
+            lo[d] = min(lo[d], __shfl_xor_sync(0xFFFFFFFFu, lo[d], off));
+            hi[d] = max(hi[d], __shfl_xor_sync(0xFFFFFFFFu, hi[d], off));
+            clo[d] = min(clo[d], __shfl_xor_sync(0xFFFFFFFFu, clo[d], off));
+            chi[d] = max(chi[d], __shfl_xor_sync(0xFFFFFFFFu, chi[d], off));
         }
         if ((threadIdx.x & 31u) == 0) {
-            atomicMin(&N.boundsLo[0][d], orderedFromFloat(lo[d]));
-            atomicMax(&N.boundsHi[0][d], orderedFromFloat(hi[d]));
-            atomicMin(&N.boundsLo[1][d], orderedFromFloat(clo[d]));
-            atomicMax(&N.boundsHi[1][d], orderedFromFloat(chi[d]));
+            atomicMin(&N.boundsLo[0][d], lo[d]);
+            atomicMax(&N.boundsHi[0][d], hi[d]);
+            atomicMin(&N.boundsLo[1][d], clo[d]);
+            atomicMax(&N.boundsHi[1][d], chi[d]);
         }
     }
 }

@@ -11,6 +11,7 @@
 // brute-force closest-hit over all triangles (BVH-independent definition of the answer).
 #pragma once
 #include "vecmath.h"
+#include <string>
 #include <vector>
 
 namespace orc {
@@ -83,6 +84,15 @@ void nodeSetChildAabb(InternalNode8 &n, uint32_t slot, const AABB &box);
 void nodeSetInvalidChildBox(InternalNode8 &n, uint32_t slot);
 
 void buildGeometryBVH(const Geometry* geoms, uint32_t numGeoms, const BuildConfig &cfg, GeometryBVH* bvh);
+
+// gpu_bvh.cpp: the world-space TriangleStorage of the geometries in order (calcTriangleVertices), and the tree the CUDA
+// builder (gfxexp_b200/csrc/bvh_build.cu) emits for gfx_bvh_build flags `flags` (binned SAH, or LBVH with
+// GFX_BVH_BUILD_FAST; PLOC is refused with -1).  sahLevels receives { small, big, huge } node counts per SAH level.
+std::vector<TriangleStorage> flattenTriangles(const Geometry* geoms, uint32_t numGeoms);
+int buildGpuStyleBVH(const Geometry* geoms, uint32_t numGeoms, uint32_t flags, GeometryBVH* bvh, std::vector<uint32_t>* sahLevels);
+// "" if both trees have the same shape, node fields (all but the two base indices) and leaf references, else the first
+// difference as a slot path from the root
+std::string sameTree(const GeometryBVH &a, const GeometryBVH &b);
 
 bool testRayVsTriangle(
     const float3 &rayOrg, const float3 &rayDir, float distMin, float distMax,

@@ -55,6 +55,15 @@ void orc_bvh_import(orc_scene* s, const GfxBvhNode8* nodes, uint32_t numNodes,
 /* structural validation of a BVH in the reference layout: every triangle referenced at least
  * once, every child box contains its subtree, leaf chains terminated. returns 0 if valid. */
 int orc_bvh_validate(orc_scene* s, char* msg, size_t msgLen);
+/* replace the BVH by the tree gfx_bvh_build(flags) builds on the GPU (gpu_bvh.cpp: binned SAH, or LBVH with
+ * GFX_BVH_BUILD_FAST); -1 for GFX_BVH_BUILD_PLOC.  Works on a scene created without an SBVH build. */
+int orc_bvh_build_gpu_style(orc_scene* s, uint32_t flags);
+/* { small, big, huge } node counts of each level of the last SAH build above (at most maxLevels triples); returns the
+ * number of levels */
+uint32_t orc_bvh_sah_levels(orc_scene* s, uint32_t* counts, uint32_t maxLevels);
+/* 0 if the two BVHs are the same tree: walked from the roots in parallel, every node field except the two base indices
+ * and every leaf's reference words are equal; else 1 and the first difference, as a slot path from the root, in msg */
+int orc_bvh_same_tree(orc_scene* a, orc_scene* b, char* msg, size_t msgLen);
 void orc_trace(orc_scene* s, const GfxRay* rays, uint32_t numRays, GfxHitObject* hits, int mode,
                OrcTraversalStats* stats, int numThreads);
 void orc_light_dist_export(orc_scene* s, float* instWeights, float* instCdf, float* integral);

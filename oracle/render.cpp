@@ -46,6 +46,7 @@ struct orc_scene {
     // flattened geometry g -> (instance, mesh slot)
     std::vector<uint32_t> geomToInst, geomToMesh;
     GeometryBVH bvh;
+    std::vector<uint32_t> sahLevels; // { small, big, huge } nodes per level of the last orc_bvh_build_gpu_style SAH build
     std::vector<float> instWeights, instCdf; // lightInstDist
     float instIntegral = 0.0f;
     double buildSeconds = 0.0;
@@ -111,12 +112,10 @@ static void buildLightDistributions(orc_scene* s) {
     s->instIntegral = exclusiveScan(s->instWeights, s->instCdf);
 }
 
-// world-space side of the scene: flattened geometry, BVH, bounds, light distributions
-static void rebuildWorld(orc_scene* s, int numThreads) {
-    const OrcBuildConfig* cfg = &s->buildConfig;
+// (instance, mesh) pairs flattened into bvh::Geometry records in instance order
+static std::vector<Geometry> collectGeometries(orc_scene* s) {
     s->geomToInst.clear();
     s->geomToMesh.clear();
-    s->bvh = GeometryBVH();
     const uint32_t numInstances = (uint32_t)s->instances.size();
     // flatten (instance, mesh) pairs into bvh::Geometry records in instance order
     std::vector<Geometry> geoms;
@@ -137,6 +136,28 @@ static void rebuildWorld(orc_scene* s, int numThreads) {
             s->geomToMesh.push_back(meshSlot);
         }
     }
+    return geoms;
+}
+
+static void updateSceneBounds(orc_scene* s) {
+    AABB box;
+    for (const TriangleStorage &ts : s->bvh.triStorages) {
+        box.unify(float3(ts.pA[0], ts.pA[1], ts.pA[2]));
+        box.unify(float3(ts.pB[0], ts.pB[1], ts.pB[2]));
+        box.unify(float3(ts.pC[0], ts.pC[1], ts.pC[2]));
+    }
+    for (int i = 0; i < 3; ++i) {
+        s->sceneMin[i] = box.minP[i];
+        s->sceneMax[i] = box.maxP[i];
+    }
+}
+
+// world-space side of the scene: flattened geometry, BVH, bounds, light distributions
+static void rebuildWorld(orc_scene* s, int numThreads) {
+    const OrcBuildConfig* cfg = &s->buildConfig;
+    s->bvh = GeometryBVH();
+    s->sahLevels.clear();
+    const std::vector<Geometry> geoms = collectGeometries(s);
     BuildConfig bc;
     bc.splittingBudget = cfg->splittingBudget;
     bc.intNodeTravCost = cfg->intNodeTravCost;
@@ -150,18 +171,35 @@ static void rebuildWorld(orc_scene* s, int numThreads) {
         buildGeometryBVH(geoms.data(), (uint32_t)geoms.size(), bc, &s->bvh);
     const auto t1 = std::chrono::steady_clock::now();
     s->buildSeconds = std::chrono::duration<double>(t1 - t0).count();
-
-    AABB box;
-    for (const TriangleStorage &ts : s->bvh.triStorages) {
-        box.unify(float3(ts.pA[0], ts.pA[1], ts.pA[2]));
-        box.unify(float3(ts.pB[0], ts.pB[1], ts.pB[2]));
-        box.unify(float3(ts.pC[0], ts.pC[1], ts.pC[2]));
-    }
-    for (int i = 0; i < 3; ++i) {
-        s->sceneMin[i] = box.minP[i];
-        s->sceneMax[i] = box.maxP[i];
-    }
+    updateSceneBounds(s);
     buildLightDistributions(s);
+}
+
+// the tree gfx_bvh_build(flags) emits (gpu_bvh.cpp) replaces the scene's BVH; works on a scene created without an SBVH
+extern "C" int orc_bvh_build_gpu_style(orc_scene* s, uint32_t flags) {
+    const std::vector<Geometry> geoms = collectGeometries(s);
+    GeometryBVH bvh;
+    std::vector<uint32_t> levels;
+    const auto t0 = std::chrono::steady_clock::now();
+    if (buildGpuStyleBVH(geoms.data(), (uint32_t)geoms.size(), flags, &bvh, &levels) != 0)
+        return -1;
+    s->buildSeconds = std::chrono::duration<double>(std::chrono::steady_clock::now() - t0).count();
+    s->bvh = std::move(bvh);
+    s->sahLevels = std::move(levels);
+    updateSceneBounds(s);
+    return 0;
+}
+extern "C" uint32_t orc_bvh_sah_levels(orc_scene* s, uint32_t* counts, uint32_t maxLevels) {
+    const uint32_t numLevels = (uint32_t)(s->sahLevels.size() / 3);
+    if (counts)
+        std::memcpy(counts, s->sahLevels.data(), 3 * (size_t)std::min(numLevels, maxLevels) * 4);
+    return numLevels;
+}
+extern "C" int orc_bvh_same_tree(orc_scene* a, orc_scene* b, char* msg, size_t msgLen) {
+    const std::string d = sameTree(a->bvh, b->bvh);
+    if (msgLen)
+        snprintf(msg, msgLen, "%s", d.c_str());
+    return d.empty() ? 0 : 1;
 }
 
 extern "C" orc_scene* orc_scene_create(const GfxSceneDesc* d, const OrcBuildConfig* cfg, int numThreads) {

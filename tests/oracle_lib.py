@@ -67,6 +67,12 @@ def lib() -> C.CDLL:
         L.orc_bvh_import.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32]
         L.orc_bvh_validate.restype = C.c_int
         L.orc_bvh_validate.argtypes = [vp, C.c_char_p, C.c_size_t]
+        L.orc_bvh_build_gpu_style.restype = C.c_int
+        L.orc_bvh_build_gpu_style.argtypes = [vp, C.c_uint32]
+        L.orc_bvh_sah_levels.restype = C.c_uint32
+        L.orc_bvh_sah_levels.argtypes = [vp, vp, C.c_uint32]
+        L.orc_bvh_same_tree.restype = C.c_int
+        L.orc_bvh_same_tree.argtypes = [vp, vp, C.c_char_p, C.c_size_t]
         L.orc_trace.argtypes = [vp, vp, C.c_uint32, vp, C.c_int, C.POINTER(OrcTraversalStats), C.c_int]
         L.orc_light_dist_export.argtypes = [vp, vp, vp, C.POINTER(C.c_float)]
         L.orc_present.argtypes = [vp, C.c_uint32, C.c_uint32, C.POINTER(abi.GfxPresentParams), vp]
@@ -189,6 +195,22 @@ class OracleScene:
         buf = C.create_string_buffer(512)
         rc = lib().orc_bvh_validate(self.h, buf, 512)
         return "" if rc == 0 else f"[{rc}] {buf.value.decode()}"
+
+    def build_gpu_style(self, flags: int = 0) -> np.ndarray:
+        """replace the BVH by the CPU restatement of the tree gfx_bvh_build(flags) builds (oracle/gpu_bvh.cpp: binned SAH,
+        or LBVH with GFX_BVH_BUILD_FAST); returns the {small, big, huge} node counts of every SAH level as [levels, 3]"""
+        assert lib().orc_bvh_build_gpu_style(self.h, flags) == 0, "PLOC has no restatement"
+        num = lib().orc_bvh_sah_levels(self.h, None, 0)
+        levels = np.zeros((num, 3), dtype=np.uint32)
+        lib().orc_bvh_sah_levels(self.h, levels.ctypes.data, num)
+        return levels
+
+    def same_tree(self, other: "OracleScene") -> str:
+        """"" if this BVH and other's are the same tree (every node field but the two base indices, every leaf's reference
+        words), else the first difference as a slot path from the root"""
+        buf = C.create_string_buffer(512)
+        rc = lib().orc_bvh_same_tree(self.h, other.h, buf, 512)
+        return "" if rc == 0 else buf.value.decode()
 
     def trace(self, rays: np.ndarray, mode: int = TRACE_CANONICAL, want_stats: bool = False, threads: int = 0):
         rays = np.ascontiguousarray(rays)

@@ -1,9 +1,10 @@
 """BASELINE.json's full size (config 2: 2.87 M triangles, 1106 instances, 1920x1080), where the CPU oracle is too slow to
 be the checker: size-independent properties of the CUDA path instead.
-  * the GPU-built BVH passes the oracle's structural validation (every triangle referenced, boxes contain subtrees);
-  * closest hits do not depend on the BVH: PLOC tree == LBVH tree, bit for bit, on primary + random rays (the canonical
-    tie-break makes the answer a function of the triangles alone);
-  * any-hit answers agree between the two trees;
+  * the three GPU-built BVHs (SAH, PLOC, LBVH) pass the oracle's structural validation (every triangle referenced, boxes
+    contain subtrees), and the SAH and LBVH trees equal their CPU restatement node for node (oracle/gpu_bvh.cpp);
+  * closest hits do not depend on the BVH: SAH tree == PLOC tree == LBVH tree, bit for bit, on primary + random rays (the
+    canonical tie-break makes the answer a function of the triangles alone);
+  * any-hit answers agree between the three trees;
   * a ReSTIR frame sequence is deterministic and equals the same sequence rendered as three row strips;
   * a sample of pixels of the first frame equals the oracle evaluated on just those rows (80-row strip), and so do three
     accumulated frames with temporal + spatial reuse (160-row strip, the 40 rows whose history stays inside it)."""
@@ -47,24 +48,35 @@ def test_config2_full_size_properties(gfx_ctx, oracle):
     rays = np.concatenate([rays, extra])
 
     results = {}
+    exported = {}
     for tag, flags in (("sah", 0), ("ploc", 0x200), ("lbvh", BVH_BUILD_FAST)):
         gfx_ctx.build_bvh(flags)
         info = gfx_ctx.bvh_info()
         assert info.numTriangles == scene.num_triangles == info.numPrimRefs
         results[tag] = (gfx_ctx.trace(rays, abi.TRACE_CLOSEST), gfx_ctx.trace(rays, abi.TRACE_ANY))
-        if tag == "ploc":
-            nodes, refs, tris = gfx_ctx.export_bvh()
-    a, b = results["ploc"][0], results["lbvh"][0]
-    for field in ("dist", "primIndex", "geomIndex", "instIndex", "bcB", "bcC"):
-        assert np.array_equal(a[field].view(np.uint32), b[field].view(np.uint32)), f"closest hits differ between builders in {field}"
-    assert np.array_equal(results["ploc"][1]["dist"].view(np.uint32), results["lbvh"][1]["dist"].view(np.uint32)), "visibility differs"
+        exported[tag] = gfx_ctx.export_bvh()
+    a = results["ploc"][0]
+    for tag in ("sah", "lbvh"):
+        b = results[tag][0]
+        for field in ("dist", "primIndex", "geomIndex", "instIndex", "bcB", "bcC"):
+            assert np.array_equal(a[field].view(np.uint32), b[field].view(np.uint32)), f"closest hits differ between PLOC and {tag} in {field}"
+        assert np.array_equal(results["ploc"][1]["dist"].view(np.uint32), results[tag][1]["dist"].view(np.uint32)), f"visibility differs ({tag})"
     assert 0.5 < float((a["primIndex"] != 0xFFFFFFFF).mean()) <= 1.0
 
-    # structural validation of the PLOC tree by the oracle's checker (no oracle BVH build: import only)
+    # structural validation of all three trees by the oracle's checker (no oracle SBVH build: import only), and the SAH (its
+    # huge nodes take the multi-block split) and LBVH trees node for node against their CPU restatement (oracle/gpu_bvh.cpp)
+    restated = oracle.OracleScene(scene, build_bvh=False)
+    for tag, flags in (("sah", 0), ("lbvh", BVH_BUILD_FAST), ("ploc", 0x200)):
+        checker = oracle.OracleScene(scene, build_bvh=False)
+        checker.import_bvh(*exported[tag])
+        assert checker.validate() == "", tag
+        if tag != "ploc":
+            levels = restated.build_gpu_style(flags)
+            assert tag == "lbvh" or levels[:, 2].max() >= 2, levels[:6]
+            diff = restated.same_tree(checker)
+            assert diff == "", f"GPU {tag} tree differs from the restatement at {diff}"
+    nodes, refs, tris = exported["ploc"]
     gfx_ctx.build_bvh(0)
-    checker = oracle.OracleScene(scene, build_bvh=False)
-    checker.import_bvh(nodes, refs, tris)
-    assert checker.validate() == ""
     # and the restated CPU traverser walking the GPU tree agrees with the GPU traverser on a sample of the rays
     sample = rays[::97].copy()
     cpu_hits = checker.trace(sample, oracle.TRACE_CANONICAL)
