@@ -101,6 +101,7 @@ assert NODE_DTYPE.itemsize == 80 and TRI_DTYPE.itemsize == 48 and HIT_DTYPE.item
 TRACE_CLOSEST, TRACE_ANY, TRACE_STATS = 0, 1, 2
 PT_BASELINE, PT_NRC, PT_REGIR = 0, 1, 2  # GfxPathTraceVariant
 NRC_READ_MASTER, NRC_READ_TRAINING, NRC_READ_INFERENCE, NRC_READ_GRADIENTS = 0, 1, 2, 3  # gfx_nrc_read
+NRC_POSITION_ENCODING_TRIANGLE_WAVE, NRC_POSITION_ENCODING_HASH_GRID = 0, 1  # gfx_nrc_create_with_encoding (PositionEncoding)
 (RESTIR_INITIAL_RIS, RESTIR_INITIAL_AND_TEMPORAL_BIASED, RESTIR_INITIAL_AND_TEMPORAL_UNBIASED,
  RESTIR_SPATIAL_BIASED, RESTIR_SPATIAL_UNBIASED, RESTIR_SHADING, RESTIR_PRESAMPLE_LIGHTS, RESTIR_PER_PIXEL_RIS,
  RESTIR_TRACE_SHADOW_RAYS, RESTIR_SHADE_AND_RESAMPLE) = range(10)
@@ -405,6 +406,7 @@ _DECLS = {
     "gfx_nrc_shuffle": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GfxFrameParams)]),
     "gfx_nrc_frame_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_float)]),
     "gfx_nrc_create": (C.c_int, [C.c_void_p, c_u32, c_f, C.POINTER(C.c_void_p)]),
+    "gfx_nrc_create_with_encoding": (C.c_int, [C.c_void_p, C.c_int, c_u32, c_f, C.POINTER(C.c_void_p)]),
     "gfx_nrc_destroy": (None, [C.c_void_p]),
     "gfx_nrc_infer": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, c_u32]),
     "gfx_nrc_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, c_u32, C.POINTER(c_f)]),

@@ -17,6 +17,11 @@
 //
 // Training (4 x 16 384 samples per frame) is latency-bound and runs on CUDA cores: one block = 128
 // samples, weights and activations in shared memory, dW reduced per block then atomically added.
+//
+// Both of NeuralRadianceCache::initialize's position encodings are built (gfx_nrc_create_with_encoding): the hash grid above,
+// and the triangle wave (triangle_wave.h:47-81), which has no parameters and no grid stage - k_nrcInferMlp<kEncTriangleWave> is
+// its whole inference, and the training kernels skip layer 0's data gradient and the encoding backward for it.  The kernels
+// are templated on the encoding; the hash-grid instantiations are the code that was here before.
 #include "context.h"
 #include <cuda_fp16.h>
 #include <random>
@@ -41,8 +46,10 @@ struct NrcLevels { NrcLevel l[kLevels]; };
 
 struct gfx_nrc {
     gfx_ctx* ctx = nullptr;
+    int positionEncoding = GFX_NRC_POSITION_ENCODING_HASH_GRID;
     uint32_t numHiddenLayers = 2;
     float learningRate = 1e-2f;
+    float adamEpsilon = 1e-15f;   // network_interface.cu:94 (triangle wave 1e-8), :119 (hash grid 1e-15)
     uint32_t numMatrixWeights = 0, numParams = 0;
     gfx::NrcLevels levels;
     __half* params = nullptr;     // current fp16 weights
@@ -214,6 +221,97 @@ GFX_D void nrcEncode(const NrcLevels &levels, const __half* __restrict__ table, 
         emit(4 + c, tail + 8 * c);
 }
 
+// triangle_wave_encoding (tiny-cuda-nn encodings/triangle_wave.h:47-81), frequency f of one position coordinate.  The only
+// products, f * 0.25f and |.| * 4, are exact, so FMA contraction cannot change the result.
+GFX_D float nrcTriangleWave(float p, uint32_t f) {
+    const float x = scalbnf(p, (int)f - 1);
+    const float val = x + (float)f * 0.25f;
+    return fabsf(val - floorf(val) - 0.5f) * 4 - 1;
+}
+
+// quartic_cdf (common_device.h:478-483) as the reference's own tiny-cuda-nn build evaluates it: nvcc contracts its polynomial
+// into three FMAs (the triangle-wave network is pinned bit for bit against that build, tests/golden/tcnn_nrc_triwave.npz)
+GFX_D float quarticCdfContracted(float x, float invRadius) {
+    const float u = x * invRadius;
+    const float u2 = u * u;
+    const float u4 = u2 * u2;
+    const float inner = __fmaf_rn(1.0f / 5.0f, u4, __fmaf_rn(-(2.0f / 3.0f), u2, 1.0f));
+    return fmaxf(0.0f, fminf(1.0f, __fmaf_rn((15.0f / 16.0f) * u, inner, 0.5f)));
+}
+
+// The triangle-wave network's one-blob + identity (q = the 14 query floats).  TriangleWave prefers the AoS layout, so the
+// Composite encoding runs every nested encoding in AoS (composite.h:253-262) and OneBlob takes kernel_one_blob (oneblob.h:83-108)
+// with one_blob_subwarp_aligned (:47-69): the CDF at the four left bin boundaries k / 4, each summed over the three periodic
+// images; bin k < 3 ends at bin k + 1's left CDF, the last bin at "bin 0's left CDF + 1".  Identity is x * 1 + 0 (identity.h:67).
+GFX_D void nrcEncodeTailAos(const float* q, __half* tail) {
+#pragma unroll
+    for (uint32_t d = 0; d < 5; ++d) {
+        const float x = q[3 + d];
+        float cdf[4];
+#pragma unroll
+        for (uint32_t k = 0; k < 4; ++k) {
+            const float left = 0.25f * (float)k; // scalbnf(k, -2)
+            cdf[k] = quarticCdfContracted(left - x, 4.0f) + quarticCdfContracted(left - x - 1.0f, 4.0f) +
+                     quarticCdfContracted(left - x + 1.0f, 4.0f);
+        }
+#pragma unroll
+        for (uint32_t k = 0; k < 4; ++k)
+            tail[d * 4 + k] = __float2half((k < 3 ? cdf[k + 1] : cdf[0] + 1.0f) - cdf[k]);
+    }
+#pragma unroll
+    for (uint32_t d = 0; d < 6; ++d)
+        tail[20 + d] = __float2half(q[8 + d] + 0.0f);
+}
+
+// The triangle-wave network's 64 inputs from the 14 query floats, in registers, delivered 8 at a time like nrcEncode:
+// TriangleWave(3 dims x 12 frequencies) feature-major in 0..35 (input 12 d + f), then one-blob 36..55 and identity 56..61,
+// and the ones Composite pads the last nested encoding with (composite.h:100-111, 231-237) in 62..63.  OneBlob's min_alignment
+// of 4 divides 36, so nothing is padded between the triangle wave and the one-blob.
+template <typename Emit>
+GFX_D void nrcEncodeTriWave(const float (&q)[kInputDims], Emit emit) {
+    __half feat[64];
+#pragma unroll
+    for (uint32_t d = 0; d < 3; ++d)
+#pragma unroll
+        for (uint32_t f = 0; f < 12; ++f)
+            feat[12 * d + f] = __float2half(nrcTriangleWave(q[d], f));
+    __half tail[26];
+    nrcEncodeTailAos(q, tail);
+#pragma unroll
+    for (uint32_t k = 0; k < 26; ++k)
+        feat[36 + k] = tail[k];
+    feat[62] = feat[63] = __float2half(1.0f);
+#pragma unroll
+    for (uint32_t c = 0; c < 8; ++c)
+        emit(c, feat + 8 * c);
+}
+
+// the network's input encoding of one query read from global memory (the kernels are templated on the encoding)
+constexpr uint32_t kEncTriangleWave = GFX_NRC_POSITION_ENCODING_TRIANGLE_WAVE, kEncHashGrid = GFX_NRC_POSITION_ENCODING_HASH_GRID;
+template <uint32_t kEnc, typename Emit>
+GFX_D void nrcEncodeQuery(const NrcLevels &levels, const __half* __restrict__ table, const float* __restrict__ in, Emit emit) {
+    if constexpr (kEnc == kEncHashGrid) {
+        nrcEncode(levels, table, in, emit);
+    }
+    else {
+        float q[kInputDims];
+#pragma unroll
+        for (uint32_t d = 0; d < kInputDims; ++d)
+            q[d] = in[d];
+        nrcEncodeTriWave(q, emit);
+    }
+}
+
+// 8 halves -> one 16-byte core-matrix row
+GFX_D uint4 packHalf8(const __half* f) {
+    uint4 v;
+    v.x = (uint32_t)__half_as_ushort(f[0]) | ((uint32_t)__half_as_ushort(f[1]) << 16);
+    v.y = (uint32_t)__half_as_ushort(f[2]) | ((uint32_t)__half_as_ushort(f[3]) << 16);
+    v.z = (uint32_t)__half_as_ushort(f[4]) | ((uint32_t)__half_as_ushort(f[5]) << 16);
+    v.w = (uint32_t)__half_as_ushort(f[6]) | ((uint32_t)__half_as_ushort(f[7]) << 16);
+    return v;
+}
+
 // ---------------------------------------------------------------------------------------------
 // wgmma helpers (PTX for sm_90a)
 // ---------------------------------------------------------------------------------------------
@@ -359,6 +457,7 @@ __global__ void k_nrcPrepWeights(const __half* __restrict__ w, uint32_t numHidde
 constexpr uint32_t kTileRows = 128;
 constexpr uint32_t kATileBytes = kTileRows * kWidth * 2; // 16 KB: 8 K-chunks x 128 rows x 16 B
 
+template <uint32_t kEnc>
 __global__ void __launch_bounds__(128) k_nrcInfer(NrcLevels levels, const __half* __restrict__ table,
                                                   const uint4* __restrict__ ummaWeights, uint32_t numHiddenLayers,
                                                   const float* __restrict__ input, float* __restrict__ output,
@@ -385,13 +484,8 @@ __global__ void __launch_bounds__(128) k_nrcInfer(NrcLevels levels, const __half
         const uint32_t row = tile * kTileRows + tid;
         // ---- encode this thread's query into the A tile: chunk c at c * 2048 + row * 16
         if (row < numData) {
-            nrcEncode(levels, table, input + (size_t)row * kInputDims, [&](uint32_t c, const __half* f) {
-                uint4 v;
-                v.x = (uint32_t)__half_as_ushort(f[0]) | ((uint32_t)__half_as_ushort(f[1]) << 16);
-                v.y = (uint32_t)__half_as_ushort(f[2]) | ((uint32_t)__half_as_ushort(f[3]) << 16);
-                v.z = (uint32_t)__half_as_ushort(f[4]) | ((uint32_t)__half_as_ushort(f[5]) << 16);
-                v.w = (uint32_t)__half_as_ushort(f[6]) | ((uint32_t)__half_as_ushort(f[7]) << 16);
-                *reinterpret_cast<uint4*>(sA + c * (kTileRows * 16) + tid * 16) = v;
+            nrcEncodeQuery<kEnc>(levels, table, input + (size_t)row * kInputDims, [&](uint32_t c, const __half* f) {
+                *reinterpret_cast<uint4*>(sA + c * (kTileRows * 16) + tid * 16) = packHalf8(f);
             });
         }
         else {
@@ -567,22 +661,29 @@ __global__ void __launch_bounds__(kEncodeThreads, 1) k_nrcGridEncode(NrcLevels l
     }
 }
 
-// queries of one tile and its grid features, landed by TMA
-struct NrcTileStage {
+// queries of one tile and, for the hash grid, its grid features, landed by TMA
+template <uint32_t kEnc> struct NrcTileStage {
     float query[128 * kInputDims];    // 7168 B
     __half2 feat[kLevels * 128];      // 8192 B
 };
+template <> struct NrcTileStage<kEncTriangleWave> { // the triangle wave is computed from the queries alone
+    float query[128 * kInputDims];
+};
 
+// k_nrcInferMlp<kEncTriangleWave> is the whole triangle-wave inference: no grid stage in front of it, the thread that owns a row
+// computes its 64 inputs from the staged query in registers.
+template <uint32_t kEnc>
 __global__ void __launch_bounds__(128) k_nrcInferMlp(const uint4* __restrict__ ummaWeights, uint32_t numHiddenLayers,
                                                      const float* __restrict__ input, const __half2* __restrict__ features,
                                                      float* __restrict__ output, uint32_t numDataImm,
                                                      const uint32_t* __restrict__ numDataPtr) {
+    using Stage = NrcTileStage<kEnc>;
     const uint32_t numData = numDataPtr ? *numDataPtr : numDataImm;
     extern __shared__ __align__(128) uint8_t smem[];
     uint8_t* sA = smem;                                                        // activation tile (A operand), 16 KB
-    NrcTileStage* stage = reinterpret_cast<NrcTileStage*>(smem + kATileBytes); // 2 x 15 KB
-    float* sOut = reinterpret_cast<float*>(smem + kATileBytes + 2 * sizeof(NrcTileStage)); // 128 x 3 floats
-    uint8_t* sW = smem + kATileBytes + 2 * sizeof(NrcTileStage) + 128 * kOutputDims * 4;   // weight blobs (B operands)
+    Stage* stage = reinterpret_cast<Stage*>(smem + kATileBytes);               // 2 x 15 KB (triangle wave: 2 x 7 KB)
+    float* sOut = reinterpret_cast<float*>(smem + kATileBytes + 2 * sizeof(Stage)); // 128 x 3 floats
+    uint8_t* sW = smem + kATileBytes + 2 * sizeof(Stage) + 128 * kOutputDims * 4;   // weight blobs (B operands)
     __shared__ __align__(8) uint64_t stageBar[2];
 
     const uint32_t tid = threadIdx.x;
@@ -591,9 +692,10 @@ __global__ void __launch_bounds__(128) k_nrcInferMlp(const uint4* __restrict__ u
 
     auto requestTile = [&](uint32_t tile, uint32_t b) { // thread 0 only
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        mbarExpectTx(&stageBar[b], (uint32_t)sizeof(NrcTileStage));
+        mbarExpectTx(&stageBar[b], (uint32_t)sizeof(Stage));
         bulkLoad(stage[b].query, input + (size_t)tile * 128 * kInputDims, 128 * kInputDims * 4, &stageBar[b]);
-        bulkLoad(stage[b].feat, features + (size_t)tile * kLevels * 128, kTileFeatureBytes, &stageBar[b]);
+        if constexpr (kEnc == kEncHashGrid)
+            bulkLoad(stage[b].feat, features + (size_t)tile * kLevels * 128, kTileFeatureBytes, &stageBar[b]);
     };
 
     if (tid == 0) {
@@ -623,19 +725,28 @@ __global__ void __launch_bounds__(128) k_nrcInferMlp(const uint4* __restrict__ u
             mbarWait(&stageBar[1], stagePhase1);
             stagePhase1 ^= 1u;
         }
-        const NrcTileStage &st = stage[buf];
+        const Stage &st = stage[buf];
 
         // ---- this thread's row of the A tile: chunk c (8 features = 16 B) at c * 2048 + row * 16
+        if constexpr (kEnc == kEncTriangleWave) {
+            float q[kInputDims];
 #pragma unroll
-        for (uint32_t c = 0; c < 4; ++c) { // hash grid: levels 4c .. 4c + 3
-            uint4 v;
-            v.x = *reinterpret_cast<const uint32_t*>(&st.feat[(4 * c + 0) * 128 + tid]);
-            v.y = *reinterpret_cast<const uint32_t*>(&st.feat[(4 * c + 1) * 128 + tid]);
-            v.z = *reinterpret_cast<const uint32_t*>(&st.feat[(4 * c + 2) * 128 + tid]);
-            v.w = *reinterpret_cast<const uint32_t*>(&st.feat[(4 * c + 3) * 128 + tid]);
-            *reinterpret_cast<uint4*>(sA + c * (kTileRows * 16) + tid * 16) = v;
+            for (uint32_t d = 0; d < kInputDims; ++d)
+                q[d] = st.query[tid * kInputDims + d];
+            nrcEncodeTriWave(q, [&](uint32_t c, const __half* f) {
+                *reinterpret_cast<uint4*>(sA + c * (kTileRows * 16) + tid * 16) = packHalf8(f);
+            });
         }
-        {
+        else {
+#pragma unroll
+            for (uint32_t c = 0; c < 4; ++c) { // hash grid: levels 4c .. 4c + 3
+                uint4 v;
+                v.x = *reinterpret_cast<const uint32_t*>(&st.feat[(4 * c + 0) * 128 + tid]);
+                v.y = *reinterpret_cast<const uint32_t*>(&st.feat[(4 * c + 1) * 128 + tid]);
+                v.z = *reinterpret_cast<const uint32_t*>(&st.feat[(4 * c + 2) * 128 + tid]);
+                v.w = *reinterpret_cast<const uint32_t*>(&st.feat[(4 * c + 3) * 128 + tid]);
+                *reinterpret_cast<uint4*>(sA + c * (kTileRows * 16) + tid * 16) = v;
+            }
             float q[kInputDims];
             q[0] = q[1] = q[2] = 0.0f;
 #pragma unroll
@@ -644,15 +755,8 @@ __global__ void __launch_bounds__(128) k_nrcInferMlp(const uint4* __restrict__ u
             __half tail[32];
             nrcEncodeTail(q, tail);
 #pragma unroll
-            for (uint32_t c = 0; c < 4; ++c) {
-                uint4 v;
-                const __half* f = tail + 8 * c;
-                v.x = (uint32_t)__half_as_ushort(f[0]) | ((uint32_t)__half_as_ushort(f[1]) << 16);
-                v.y = (uint32_t)__half_as_ushort(f[2]) | ((uint32_t)__half_as_ushort(f[3]) << 16);
-                v.z = (uint32_t)__half_as_ushort(f[4]) | ((uint32_t)__half_as_ushort(f[5]) << 16);
-                v.w = (uint32_t)__half_as_ushort(f[6]) | ((uint32_t)__half_as_ushort(f[7]) << 16);
-                *reinterpret_cast<uint4*>(sA + (4 + c) * (kTileRows * 16) + tid * 16) = v;
-            }
+            for (uint32_t c = 0; c < 4; ++c)
+                *reinterpret_cast<uint4*>(sA + (4 + c) * (kTileRows * 16) + tid * 16) = packHalf8(tail + 8 * c);
         }
 
         for (uint32_t layer = 0; layer <= numHiddenLayers; ++layer) {
@@ -720,6 +824,20 @@ __global__ void k_nrcAssembleEncoding(const float* __restrict__ input, const __h
         o[32 + k] = tail[k];
 }
 
+// test hook: the triangle-wave network's 64 inputs per query, by the nrcEncodeTriWave the inference kernels run
+__global__ void k_nrcTriWaveEncoding(const float* __restrict__ input, uint32_t numData, __half* __restrict__ out) {
+    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
+    if (q >= numData)
+        return;
+    float qv[kInputDims];
+    for (uint32_t d = 0; d < kInputDims; ++d)
+        qv[d] = input[(size_t)q * kInputDims + d];
+    nrcEncodeTriWave(qv, [&](uint32_t c, const __half* f) {
+        for (uint32_t e = 0; e < 8; ++e)
+            out[(size_t)q * 64 + c * 8 + e] = f[e];
+    });
+}
+
 // ---------------------------------------------------------------------------------------------
 // training step on CUDA cores: block = 128 samples
 // ---------------------------------------------------------------------------------------------
@@ -734,6 +852,9 @@ GFX_D float fixedToFloat(unsigned long long v) {
 
 constexpr uint32_t kRowStride = 66; // halves per activation row in shared memory (conflict-free rows)
 
+// kEnc = kEncTriangleWave: the encoding has no parameters, so NetworkWithInputEncoding::backward asks for no input gradient
+// (network_with_input_encoding.h:92-99): no data gradient through layer 0 and no encoding backward
+template <uint32_t kEnc>
 __global__ void __launch_bounds__(128) k_nrcTrain(NrcLevels levels, const __half* __restrict__ params, uint32_t numMatrixWeights,
                                                   uint32_t numHiddenLayers, const float* __restrict__ input,
                                                   const float* __restrict__ target, uint32_t numData,
@@ -754,7 +875,7 @@ __global__ void __launch_bounds__(128) k_nrcTrain(NrcLevels levels, const __half
 
     __half* x = sAct + (size_t)tid * kRowStride;
     if (valid) {
-        nrcEncode(levels, table, input + (size_t)q * kInputDims, [&](uint32_t c, const __half* f) {
+        nrcEncodeQuery<kEnc>(levels, table, input + (size_t)q * kInputDims, [&](uint32_t c, const __half* f) {
 #pragma unroll
             for (uint32_t e = 0; e < 8; ++e)
                 x[c * 8 + e] = f[e];
@@ -849,6 +970,8 @@ __global__ void __launch_bounds__(128) k_nrcTrain(NrcLevels levels, const __half
             if (acc != 0.0f)
                 atomicAddFixed(grads + base + p, acc);
         }
+        if (kEnc == kEncTriangleWave && layer == 0)
+            break;
         const __half* W = sW + (size_t)layer * kWidth * kWidth;
         const __half* myIn = hin + (size_t)tid * kRowStride;
         __half dNext[64];
@@ -865,7 +988,7 @@ __global__ void __launch_bounds__(128) k_nrcTrain(NrcLevels levels, const __half
     }
 
     // hash-grid backward (kernel_grid_backward, grid.h:306-429): scatter the first 32 input gradients
-    if (valid) {
+    if (kEnc == kEncHashGrid && valid) {
         unsigned long long* gGrid = grads + numMatrixWeights;
         const float* in = input + (size_t)q * kInputDims;
         for (uint32_t l = 0; l < kLevels; ++l) {
@@ -945,6 +1068,7 @@ __global__ void k_nrcPrepTrainWeights(const __half* __restrict__ w, uint32_t num
     }
 }
 
+template <uint32_t kEnc> // as k_nrcTrain: the triangle wave skips layer 0's data gradient and the encoding backward
 __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __half* __restrict__ params, uint32_t numMatrixWeights,
                                                     uint32_t numHiddenLayers, const uint4* __restrict__ blobFwd,
                                                     const uint4* __restrict__ blobT, const float* __restrict__ input,
@@ -980,7 +1104,7 @@ __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __ha
 
     // encode this thread's sample into A_0
     if (valid) {
-        nrcEncode(levels, table, input + (size_t)q * kInputDims, [&](uint32_t c, const __half* f) {
+        nrcEncodeQuery<kEnc>(levels, table, input + (size_t)q * kInputDims, [&](uint32_t c, const __half* f) {
             uint4 v;
             v.x = (uint32_t)__half_as_ushort(f[0]) | ((uint32_t)__half_as_ushort(f[1]) << 16);
             v.y = (uint32_t)__half_as_ushort(f[2]) | ((uint32_t)__half_as_ushort(f[3]) << 16);
@@ -1109,6 +1233,8 @@ __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __ha
                             atomicAddFixed(grads + base + r * kWidth + c, g);
                     }
         }
+        if (kEnc == kEncTriangleWave && layer == 0)
+            break;
         // data gradient dA_l = dZ_l x W_l (K steps of 16 over dZ's width) -> dZ_{l-1} (ReLU mask of A_l = relu(Z_{l-1})), or
         // the encoder gradient for layer 0, written over dZ_l
         {
@@ -1133,7 +1259,7 @@ __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __ha
 
     // ---- hash-grid backward (kernel_grid_backward, grid.h:306-429): scatter the first 32 input gradients (this sample's
     // row of the dZ tile)
-    if (valid) {
+    if (kEnc == kEncHashGrid && valid) {
         unsigned long long* gGrid = grads + numMatrixWeights;
         const float* in = input + (size_t)q * kInputDims;
         for (uint32_t l = 0; l < kLevels; ++l) {
@@ -1172,14 +1298,14 @@ __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __ha
 }
 
 // adam_step (adam.h:49-115) + ema_step_half_precision (ema.h:61-77); clears the gradient for the next step
-__global__ void k_nrcAdamEma(uint32_t numParams, uint32_t numMatrixWeights, float learningRate, float emaDebiasOld,
+__global__ void k_nrcAdamEma(uint32_t numParams, uint32_t numMatrixWeights, float learningRate, float epsilon, float emaDebiasOld,
                              float emaDebiasNew, unsigned long long* __restrict__ grads, float* __restrict__ master,
                              __half* __restrict__ params, __half* __restrict__ paramsEma, float* __restrict__ m1,
                              float* __restrict__ m2, uint32_t* __restrict__ steps) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= numParams)
         return;
-    const float beta1 = 0.9f, beta2 = 0.99f, epsilon = 1e-15f, l2Reg = 1e-6f, emaDecay = 0.99f;
+    const float beta1 = 0.9f, beta2 = 0.99f, l2Reg = 1e-6f, emaDecay = 0.99f;
     float gradient = __half2float(__float2half(fixedToFloat(grads[i]))) / kLossScale;
     grads[i] = 0ull;
     const bool matrix = i < numMatrixWeights;
@@ -1235,7 +1361,8 @@ static void setupLevels(gfx_nrc* n) { // grid.h:885-922
         offset += paramsInLevel;
     }
     n->numMatrixWeights = kWidth * kWidth * n->numHiddenLayers + kPaddedOutput * kWidth;
-    n->numParams = n->numMatrixWeights + offset * 2;
+    // the triangle-wave encoding has no parameters (triangle_wave.h: n_params() == 0)
+    n->numParams = n->numMatrixWeights + (n->positionEncoding == GFX_NRC_POSITION_ENCODING_HASH_GRID ? offset * 2 : 0u);
 }
 
 // tiny-cuda-nn's pcg32 (dependencies/pcg32/pcg32.h:46-116): 64-bit LCG, XSH-RR output
@@ -1268,7 +1395,8 @@ struct Pcg32 {
 // scale = sqrt(6 / (fan_in + fan_out)) (fully_fused_mlp.cu:922-949, gpu_matrix.h:292-307) - then the encoding: the hash grid
 // U(-1e-4, 1e-4) by generate_random_uniform (grid.h:1267-1272, random.h:65-100), a kernel in which thread i jumps the stream
 // ahead by 4 i and writes elements i, i + T, i + 2T, i + 3T (T = total threads) with val * (upper - lower) + lower, one FMA
-// under nvcc's default contraction.  One-blob and identity have no parameters.
+// under nvcc's default contraction.  One-blob, identity and the triangle wave have no parameters: for a triangle-wave network
+// numParams == numMatrixWeights and nothing is drawn after the matrices.
 static void tcnnInitialParams(uint32_t seed, uint32_t numHiddenLayers, uint32_t numMatrixWeights, uint32_t numParams,
                               std::vector<float>* master) {
     std::seed_seq seq{ seed };
@@ -1284,6 +1412,8 @@ static void tcnnInitialParams(uint32_t seed, uint32_t numHiddenLayers, uint32_t 
             (*master)[pos++] = rng.nextFloat() * 2.0f * scale - scale;
     }
     const size_t n = numParams - numMatrixWeights;
+    if (n == 0) // no encoding parameters: no generate_random_uniform
+        return;
     const size_t threadsNeeded = (n + 3) / 4;
     const size_t totalThreads = (threadsNeeded + 127) / 128 * 128; // n_blocks_linear(n_threads) * n_threads_linear
     std::vector<float> stream(totalThreads * 4);
@@ -1303,8 +1433,9 @@ static void tcnnInitialParams(uint32_t seed, uint32_t numHiddenLayers, uint32_t 
 // gfx_nrc_create rejects a depth for which one of them exceeds the device's per-block limit.
 constexpr uint32_t kMaxTcTrainHiddenLayers = 3; // deeper networks train on k_nrcTrain
 static size_t nrcInferFusedSmem(uint32_t numMatrixWeights) { return kATileBytes + (size_t)numMatrixWeights * 2; }
+template <uint32_t kEnc>
 static size_t nrcInferMlpSmem(uint32_t numMatrixWeights) {
-    return kATileBytes + 2 * sizeof(NrcTileStage) + 128 * kOutputDims * 4 + (size_t)numMatrixWeights * 2;
+    return kATileBytes + 2 * sizeof(NrcTileStage<kEnc>) + 128 * kOutputDims * 4 + (size_t)numMatrixWeights * 2;
 }
 static size_t nrcTrainTcSmem(uint32_t numMatrixWeights, uint32_t numHiddenLayers) {
     return (size_t)numMatrixWeights * 4 + (size_t)(numHiddenLayers + 1) * kATileBytes + 3 * (size_t)kATileBytes;
@@ -1317,17 +1448,25 @@ static size_t nrcTrainSmem(uint32_t numMatrixWeights, uint32_t numHiddenLayers) 
 
 using namespace gfx;
 
-// every kernel that can train or infer a network of this depth fits in one block's shared memory (dynamic + static)
+struct NrcKernelSmem { const void* kernel; const char* name; size_t dynamicBytes; };
+template <uint32_t kEnc>
+static void nrcKernelSmem(uint32_t M, uint32_t H, NrcKernelSmem (&kernels)[4]) {
+    kernels[0] = { (const void*)k_nrcInfer<kEnc>, "k_nrcInfer", nrcInferFusedSmem(M) };
+    kernels[1] = { (const void*)k_nrcInferMlp<kEnc>, "k_nrcInferMlp", nrcInferMlpSmem<kEnc>(M) };
+    kernels[2] = { (const void*)k_nrcTrainTc<kEnc>, "k_nrcTrainTc", H <= kMaxTcTrainHiddenLayers ? nrcTrainTcSmem(M, H) : 0 };
+    kernels[3] = { (const void*)k_nrcTrain<kEnc>, "k_nrcTrain", nrcTrainSmem(M, H) };
+}
+
+// every kernel that can train or infer a network of this depth and encoding fits in one block's shared memory (dynamic + static)
 static int nrcCheckSharedMemory(gfx_ctx* ctx, const gfx_nrc* n) {
     int limit = 0;
     GFX_CUDA(ctx, cudaDeviceGetAttribute(&limit, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
     const uint32_t M = n->numMatrixWeights, H = n->numHiddenLayers;
-    const struct { const void* kernel; const char* name; size_t dynamicBytes; } kernels[] = {
-        { (const void*)k_nrcInfer, "k_nrcInfer", nrcInferFusedSmem(M) },
-        { (const void*)k_nrcInferMlp, "k_nrcInferMlp", nrcInferMlpSmem(M) },
-        { (const void*)k_nrcTrainTc, "k_nrcTrainTc", H <= kMaxTcTrainHiddenLayers ? nrcTrainTcSmem(M, H) : 0 },
-        { (const void*)k_nrcTrain, "k_nrcTrain", nrcTrainSmem(M, H) },
-    };
+    NrcKernelSmem kernels[4];
+    if (n->positionEncoding == GFX_NRC_POSITION_ENCODING_HASH_GRID)
+        nrcKernelSmem<kEncHashGrid>(M, H, kernels);
+    else
+        nrcKernelSmem<kEncTriangleWave>(M, H, kernels);
     for (const auto &k : kernels) {
         cudaFuncAttributes attr;
         GFX_CUDA(ctx, cudaFuncGetAttributes(&attr, k.kernel));
@@ -1352,9 +1491,18 @@ int gfx_nrc_reset(gfx_nrc* n, uint32_t seed);
 void gfx_nrc_destroy(gfx_nrc* n);
 
 int gfx_nrc_create(gfx_ctx* ctx, uint32_t numHiddenLayers, float learningRate, gfx_nrc** out) {
+    return gfx_nrc_create_with_encoding(ctx, GFX_NRC_POSITION_ENCODING_HASH_GRID, numHiddenLayers, learningRate, out);
+}
+
+int gfx_nrc_create_with_encoding(gfx_ctx* ctx, int positionEncoding, uint32_t numHiddenLayers, float learningRate,
+                                 gfx_nrc** out) {
     if (!ctx || !out)
         return GFX_ERR_INVALID_ARGUMENT;
     *out = nullptr;
+    if (positionEncoding != GFX_NRC_POSITION_ENCODING_TRIANGLE_WAVE && positionEncoding != GFX_NRC_POSITION_ENCODING_HASH_GRID) {
+        ctx->setError("gfx_nrc_create: positionEncoding must be GFX_NRC_POSITION_ENCODING_TRIANGLE_WAVE or _HASH_GRID");
+        return GFX_ERR_INVALID_ARGUMENT;
+    }
     if (numHiddenLayers < 1 || numHiddenLayers > 8) {
         ctx->setError("gfx_nrc_create: numHiddenLayers must be in 1..8");
         return GFX_ERR_INVALID_ARGUMENT;
@@ -1362,8 +1510,10 @@ int gfx_nrc_create(gfx_ctx* ctx, uint32_t numHiddenLayers, float learningRate, g
     GFX_CUDA(ctx, cudaSetDevice(ctx->device));
     gfx_nrc* n = new gfx_nrc();
     n->ctx = ctx;
+    n->positionEncoding = positionEncoding;
     n->numHiddenLayers = numHiddenLayers;
     n->learningRate = learningRate;
+    n->adamEpsilon = positionEncoding == GFX_NRC_POSITION_ENCODING_TRIANGLE_WAVE ? 1e-8f : 1e-15f;
     setupLevels(n);
     const int fits = nrcCheckSharedMemory(ctx, n);
     if (fits != GFX_OK) {
@@ -1529,17 +1679,32 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const uint32_t numTiles = numData / kTileRows; // upper bound when numDataPtr is given
-    // GFX_NRC_INFER_FUSED=1: the one-kernel form (encode by L2 gathers inside the MLP kernel), the A/B arm; it is also the
-    // path for buffers the TMA bulk copies cannot take (not 16-byte aligned)
+    // GFX_NRC_INFER_FUSED=1: the hash grid's one-kernel form (encode by L2 gathers inside the MLP kernel), the A/B arm; for both
+    // encodings it is also the path for buffers the TMA bulk copies cannot take (not 16-byte aligned)
+    const bool hashGrid = n->positionEncoding == GFX_NRC_POSITION_ENCODING_HASH_GRID;
     const char* fusedEnv = getenv("GFX_NRC_INFER_FUSED");
     const bool aligned = (reinterpret_cast<uintptr_t>(inputData) & 15u) == 0 && (reinterpret_cast<uintptr_t>(predictionData) & 15u) == 0;
-    if ((fusedEnv && fusedEnv[0] == '1') || !aligned) {
+    if ((hashGrid && fusedEnv && fusedEnv[0] == '1') || !aligned) {
         const size_t smem = nrcInferFusedSmem(n->numMatrixWeights);
-        NRC_CUDA(n, cudaFuncSetAttribute(k_nrcInfer, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        auto kernel = hashGrid ? k_nrcInfer<kEncHashGrid> : k_nrcInfer<kEncTriangleWave>;
+        NRC_CUDA(n, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         const uint32_t grid = numTiles < (uint32_t)sms * 6 ? numTiles : (uint32_t)sms * 6;
         GFX_TIMED(n->ctx, s, "nrc_infer");
-        k_nrcInfer<<<grid, 128, smem, s>>>(n->levels, n->paramsEma + n->numMatrixWeights, n->ummaWeights, n->numHiddenLayers,
-                                           inputData, predictionData, numData, numDataPtr);
+        kernel<<<grid, 128, smem, s>>>(n->levels, n->paramsEma + n->numMatrixWeights, n->ummaWeights, n->numHiddenLayers,
+                                       inputData, predictionData, numData, numDataPtr);
+        n->ctx->launches++;
+        NRC_CUDA(n, cudaGetLastError());
+        return GFX_OK;
+    }
+    if (!hashGrid) { // triangle wave: one persistent kernel, nothing in front of it
+        const size_t smem = nrcInferMlpSmem<kEncTriangleWave>(n->numMatrixWeights);
+        NRC_CUDA(n, cudaFuncSetAttribute(k_nrcInferMlp<kEncTriangleWave>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        const uint32_t ctasPerSm = (uint32_t)(220 * 1024 / (smem + 1024));
+        const uint32_t maxGrid = (uint32_t)sms * (ctasPerSm ? ctasPerSm : 1u);
+        const uint32_t grid = numTiles < maxGrid ? numTiles : maxGrid;
+        GFX_TIMED(n->ctx, s, "nrc_infer");
+        k_nrcInferMlp<kEncTriangleWave><<<grid, 128, smem, s>>>(n->ummaWeights, n->numHiddenLayers, inputData, nullptr,
+                                                                predictionData, numData, numDataPtr);
         n->ctx->launches++;
         NRC_CUDA(n, cudaGetLastError());
         return GFX_OK;
@@ -1550,13 +1715,14 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
     rc = nrcGridEncodeLaunch(n, s, inputData, numData, numDataPtr, true);
     if (rc != GFX_OK)
         return rc;
-    const size_t smem = nrcInferMlpSmem(n->numMatrixWeights);
-    NRC_CUDA(n, cudaFuncSetAttribute(k_nrcInferMlp, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = nrcInferMlpSmem<kEncHashGrid>(n->numMatrixWeights);
+    NRC_CUDA(n, cudaFuncSetAttribute(k_nrcInferMlp<kEncHashGrid>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const uint32_t ctasPerSm = (uint32_t)(220 * 1024 / (smem + 1024));
     const uint32_t maxGrid = (uint32_t)sms * (ctasPerSm ? ctasPerSm : 1u);
     const uint32_t grid = numTiles < maxGrid ? numTiles : maxGrid;
     GFX_TIMED(n->ctx, s, "nrc_infer");
-    k_nrcInferMlp<<<grid, 128, smem, s>>>(n->ummaWeights, n->numHiddenLayers, inputData, n->features, predictionData, numData, numDataPtr);
+    k_nrcInferMlp<kEncHashGrid><<<grid, 128, smem, s>>>(n->ummaWeights, n->numHiddenLayers, inputData, n->features, predictionData,
+                                                        numData, numDataPtr);
     n->ctx->launches++;
     NRC_CUDA(n, cudaGetLastError());
     return GFX_OK;
@@ -1564,6 +1730,12 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
 
 // test hook (gfx_nrc_encode_debug): the encoded network input of numData queries, [numData][64] halves, through the split path
 static int nrcEncodeDebug(gfx_nrc* n, cudaStream_t s, const float* inputData, uint32_t numData, void* outHalf) {
+    if (n->positionEncoding == GFX_NRC_POSITION_ENCODING_TRIANGLE_WAVE) {
+        k_nrcTriWaveEncoding<<<(numData + 127) / 128, 128, 0, s>>>(inputData, numData, reinterpret_cast<__half*>(outHalf));
+        n->ctx->launches++;
+        NRC_CUDA(n, cudaGetLastError());
+        return GFX_OK;
+    }
     int rc = nrcEnsureScratch(n, numData);
     if (rc != GFX_OK)
         return rc;
@@ -1672,24 +1844,26 @@ int gfx_nrc_train(gfx_nrc* n, void* stream, const float* inputData, const float*
     // networks whose activation tiles do not fit in shared memory and as the A/B switch GFX_NRC_TRAIN_CUDACORES=1.
     const char* cudaCoresEnv = getenv("GFX_NRC_TRAIN_CUDACORES");
     const bool forceCudaCores = cudaCoresEnv && cudaCoresEnv[0] == '1';
+    const bool hashGrid = n->positionEncoding == GFX_NRC_POSITION_ENCODING_HASH_GRID;
     if (n->numHiddenLayers <= kMaxTcTrainHiddenLayers && !forceCudaCores) {
         const size_t smem = nrcTrainTcSmem(n->numMatrixWeights, n->numHiddenLayers);
-        NRC_CUDA(n, cudaFuncSetAttribute(k_nrcTrainTc, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        auto kernel = hashGrid ? k_nrcTrainTc<kEncHashGrid> : k_nrcTrainTc<kEncTriangleWave>;
+        NRC_CUDA(n, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         { GFX_TIMED(n->ctx, s, "nrc_train_prep_weights");
         k_nrcPrepTrainWeights<<<32, 256, 0, s>>>(n->params, n->numHiddenLayers, reinterpret_cast<__half*>(n->trainBlobFwd),
                                                  reinterpret_cast<__half*>(n->trainBlobT)); }
         n->ctx->launches++;
         { GFX_TIMED(n->ctx, s, "nrc_train_fwd_bwd");
-        k_nrcTrainTc<<<numData / 128, 128, smem, s>>>(n->levels, n->params, n->numMatrixWeights, n->numHiddenLayers,
-                                                      n->trainBlobFwd, n->trainBlobT, inputData, targetData, numData, n->grads,
-                                                      n->loss); }
+        kernel<<<numData / 128, 128, smem, s>>>(n->levels, n->params, n->numMatrixWeights, n->numHiddenLayers, n->trainBlobFwd,
+                                                n->trainBlobT, inputData, targetData, numData, n->grads, n->loss); }
     }
     else {
         const size_t smem = nrcTrainSmem(n->numMatrixWeights, n->numHiddenLayers);
-        NRC_CUDA(n, cudaFuncSetAttribute(k_nrcTrain, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        auto kernel = hashGrid ? k_nrcTrain<kEncHashGrid> : k_nrcTrain<kEncTriangleWave>;
+        NRC_CUDA(n, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         { GFX_TIMED(n->ctx, s, "nrc_train_fwd_bwd");
-        k_nrcTrain<<<numData / 128, 128, smem, s>>>(n->levels, n->params, n->numMatrixWeights, n->numHiddenLayers, inputData,
-                                                    targetData, numData, n->grads, n->loss); }
+        kernel<<<numData / 128, 128, smem, s>>>(n->levels, n->params, n->numMatrixWeights, n->numHiddenLayers, inputData,
+                                                targetData, numData, n->grads, n->loss); }
     }
     n->ctx->launches++;
     if (n->keepGradients) {
@@ -1701,8 +1875,8 @@ int gfx_nrc_train(gfx_nrc* n, void* stream, const float* inputData, const float*
     const float emaDebiasOld = 1 - (float)pow((double)emaDecay, (double)(n->globalStep - 1));
     const float emaDebiasNew = 1.0f / (1 - (float)pow((double)emaDecay, (double)n->globalStep));
     { GFX_TIMED(n->ctx, s, "nrc_adam_ema");
-    k_nrcAdamEma<<<(n->numParams + 255) / 256, 256, 0, s>>>(n->numParams, n->numMatrixWeights, n->learningRate, emaDebiasOld,
-                                                            emaDebiasNew, n->grads, n->master, n->params, n->paramsEma,
+    k_nrcAdamEma<<<(n->numParams + 255) / 256, 256, 0, s>>>(n->numParams, n->numMatrixWeights, n->learningRate, n->adamEpsilon,
+                                                            emaDebiasOld, emaDebiasNew, n->grads, n->master, n->params, n->paramsEma,
                                                             n->m1, n->m2, n->steps); }
     n->ctx->launches++;
     n->ummaDirty = true;

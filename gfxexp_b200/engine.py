@@ -280,13 +280,18 @@ class Context:
 class NeuralRadianceCache:
     """Mirror of the reference's NeuralRadianceCache facade (neural_radiance_caching/network_interface.h:14-28):
     initialize -> __init__, infer, train, finalize -> close.  Device buffers are torch CUDA tensors or raw
-    device pointers (queries: float[numData, 14] row per query; predictions/targets: float[numData, 3])."""
+    device pointers (queries: float[numData, 14] row per query; predictions/targets: float[numData, 3]).
+    position_encoding: abi.NRC_POSITION_ENCODING_HASH_GRID (default) or _TRIANGLE_WAVE, initialize's posEnc; switching it is
+    close() + a new cache, as in the reference."""
 
-    def __init__(self, ctx: "Context", num_hidden_layers: int = 2, learning_rate: float = 1e-2):
+    def __init__(self, ctx: "Context", num_hidden_layers: int = 2, learning_rate: float = 1e-2,
+                 position_encoding: int = abi.NRC_POSITION_ENCODING_HASH_GRID):
         self.ctx = ctx
         h = C.c_void_p()
-        ctx._check(ctx.lib.gfx_nrc_create(ctx.h, num_hidden_layers, learning_rate, C.byref(h)), "gfx_nrc_create")
+        ctx._check(ctx.lib.gfx_nrc_create_with_encoding(ctx.h, position_encoding, num_hidden_layers, learning_rate, C.byref(h)),
+                   "gfx_nrc_create_with_encoding")
         self.h = h
+        self.position_encoding = position_encoding
         self.num_params = int(ctx.lib.gfx_nrc_num_params(self.h))
 
     def close(self):

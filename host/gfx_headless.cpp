@@ -7,7 +7,10 @@
 // tests/test_gpu_host_cpp.py) that the boundary is a plain C ABI: nothing here knows about Python, torch or CUDA
 // types.  Scene and default parameters come from a flat binary file written by gfxexp_b200/scenes.py::save_scene_bin.
 //
-//   gfx_headless <scene.bin> <renderer> <width> <height> <frames> <out.raw> [nrc_params.f16]
+//   gfx_headless <scene.bin> <renderer> <width> <height> <frames> <out.raw> [nrc_params.f16] [-position-encoding tri|hash]
+//   -position-encoding: the NRC network's position encoding, as the reference app's command line takes it
+//   (neural_radiance_caching_main.cpp:458, 755-766); hash grid by default.  nrc_params.f16 must hold that network's
+//   gfx_nrc_num_params halves.
 //   renderer: restir | restir_unbiased | rearch | rearch_unbiased | pathtrace | regir | nrc
 // Output: the accumulated beauty buffer (float4 per pixel, row-major) after <frames> frames, plus one line of JSON
 // with the mean milliseconds per frame (wall clock around a synchronised loop).
@@ -96,8 +99,31 @@ void loadScene(const char* path, uint32_t width, uint32_t height, SceneFile* s) 
 
 int main(int argc, char** argv) {
     if (argc < 7) {
-        fprintf(stderr, "usage: %s <scene.bin> <renderer> <width> <height> <frames> <out.raw | out.png> [nrc_params.f16]\n", argv[0]);
+        fprintf(stderr, "usage: %s <scene.bin> <renderer> <width> <height> <frames> <out.raw | out.png> [nrc_params.f16] "
+                "[-position-encoding tri|hash]\n", argv[0]);
         return 2;
+    }
+    const char* nrcParamsPath = nullptr;
+    int positionEncoding = GFX_NRC_POSITION_ENCODING_HASH_GRID;
+    for (int i = 7; i < argc; ++i) {
+        const std::string arg = argv[i];
+        if (arg == "-position-encoding" && i + 1 < argc) {
+            const std::string v = argv[++i];
+            if (v == "tri")
+                positionEncoding = GFX_NRC_POSITION_ENCODING_TRIANGLE_WAVE;
+            else if (v == "hash")
+                positionEncoding = GFX_NRC_POSITION_ENCODING_HASH_GRID;
+            else {
+                fprintf(stderr, "-position-encoding takes tri or hash, not %s\n", v.c_str());
+                return 2;
+            }
+        }
+        else if (!nrcParamsPath && arg[0] != '-')
+            nrcParamsPath = argv[i];
+        else {
+            fprintf(stderr, "unexpected argument %s\n", argv[i]);
+            return 2;
+        }
     }
     const std::string renderer = argv[2];
     const uint32_t width = (uint32_t)atoi(argv[3]), height = (uint32_t)atoi(argv[4]);
@@ -116,14 +142,19 @@ int main(int argc, char** argv) {
 
         const bool unbiased = renderer == "restir_unbiased" || renderer == "rearch_unbiased";
         if (renderer == "nrc") {
-            check(gfx, gfx_nrc_create(gfx, 2, 1e-2f, &nrc), "gfx_nrc_create");             // neuralRadianceCache.initialize
-            if (argc >= 8) {
-                FILE* pf = fopen(argv[7], "rb");
+            check(gfx, gfx_nrc_create_with_encoding(gfx, positionEncoding, 2, 1e-2f, &nrc),  // neuralRadianceCache.initialize
+                  "gfx_nrc_create_with_encoding");
+            if (nrcParamsPath) {
+                FILE* pf = fopen(nrcParamsPath, "rb");
                 if (!pf)
                     throw std::runtime_error("cannot open the NRC parameter file");
                 std::vector<uint16_t> halfParams(gfx_nrc_num_params(nrc));
-                readInto(pf, halfParams.data(), halfParams.size());
+                const size_t got = fread(halfParams.data(), 2, halfParams.size(), pf);
+                const bool longer = fgetc(pf) != EOF;
                 fclose(pf);
+                if (got != halfParams.size() || longer)
+                    throw std::runtime_error("the NRC parameter file does not hold this network's " +
+                                             std::to_string(halfParams.size()) + " halves");
                 check(gfx, gfx_nrc_set_params(nrc, halfParams.data(), halfParams.size() * 2), "gfx_nrc_set_params");
             }
         }

@@ -521,8 +521,22 @@ typedef struct gfx_nrc gfx_nrc;
  * the device's shared memory per block (cudaDevAttrMaxSharedMemoryPerBlockOptin); a deeper network is rejected with
  * GFX_ERR_UNSUPPORTED and an error string that names the kernel, its need and the limit.  On an H100 (232 448 bytes)
  * that is 1..7: at 8 the CUDA-core training kernel (the only one for more than 3 hidden layers) needs 236 544 bytes of
- * dynamic shared memory alone. */
+ * dynamic shared memory alone.  gfx_nrc_create builds the hash-grid network: it is
+ * gfx_nrc_create_with_encoding(ctx, GFX_NRC_POSITION_ENCODING_HASH_GRID, ...). */
 int gfx_nrc_create(gfx_ctx* ctx, uint32_t numHiddenLayers, float learningRate, gfx_nrc** out);
+/* NeuralRadianceCache::initialize(posEnc, numHiddenLayers, learningRate) (network_interface.cu:48-121); the values are those
+ * of PositionEncoding (network_interface.h:5-8).  The position (query floats 0..2) is encoded by
+ *   TRIANGLE_WAVE  TriangleWave(12 frequencies): network inputs 0..35, input 12 d + f of position dim d and frequency f
+ *                  (triangle_wave.h:47-81); OneBlob 36..55, Identity 56..61, ones 62..63.  The encoding has no parameters:
+ *                  numParams = the MLP's matrix weights.  Adam epsilon 1e-8.
+ *   HASH_GRID      HashGrid(16 levels x 2 features): inputs 0..31; OneBlob 32..51, Identity 52..57, ones 58..63.
+ *                  numParams = matrix weights + 991 232 grid entries.  Adam epsilon 1e-15.
+ * Any other value is GFX_ERR_INVALID_ARGUMENT.  The depth limits are the same for both.  Switching the encoding at run
+ * time is gfx_nrc_destroy + create, as in the reference. */
+#define GFX_NRC_POSITION_ENCODING_TRIANGLE_WAVE 0
+#define GFX_NRC_POSITION_ENCODING_HASH_GRID 1
+int gfx_nrc_create_with_encoding(gfx_ctx* ctx, int positionEncoding, uint32_t numHiddenLayers, float learningRate,
+                                 gfx_nrc** out);
 void gfx_nrc_destroy(gfx_nrc* nrc);
 /* inputData: device float[14, numData] (column per query), predictionData: device float[3, numData];
  * numData % 128 == 0 (network_interface.cu:141-147) */
@@ -532,7 +546,8 @@ int gfx_nrc_train(gfx_nrc* nrc, void* stream, const float* inputData, const floa
 /* gfx_nrc_create leaves the cache as NeuralRadianceCache::initialize leaves tiny-cuda-nn's Trainer (seed 1337): Xavier-uniform MLP
  * matrices and U(-1e-4, 1e-4) hash-grid entries drawn from pcg32 in tiny-cuda-nn's order (trainer.h:54-109, gpu_matrix.h:292-307,
  * grid.h:1267-1272, random.h:65-100), fp32 master = those values, training weights = their halves, inference (EMA) weights and
- * optimizer state zero.  gfx_nrc_reset re-initialises with another Trainer seed. */
+ * optimizer state zero.  gfx_nrc_reset re-initialises with another Trainer seed.  A triangle-wave network draws the same
+ * matrices (the same pcg32 prefix) and nothing after them. */
 int gfx_nrc_reset(gfx_nrc* nrc, uint32_t seed);
 /* state read-back for parity tests.  which: MASTER fp32[numParams]; TRAINING / INFERENCE half[numParams];
  * GRADIENTS fp32[numParams] = the loss-scaled (x128) gradients of the last gfx_nrc_train, rounded to half like
@@ -543,8 +558,9 @@ int gfx_nrc_reset(gfx_nrc* nrc, uint32_t seed);
 #define GFX_NRC_READ_GRADIENTS 3
 int gfx_nrc_read(gfx_nrc* nrc, int which, void* hostOut, size_t bytes);
 int gfx_nrc_keep_gradients(gfx_nrc* nrc, int on);
-/* test hook: the encoded network input (HashGrid 32 | OneBlob 20 | Identity 6 | ones 6 = 64 halves per query; kernel_grid
- * grid.h:132-255, kernel_one_blob_soa oneblob.h:110-139) of numData DEVICE queries as gfx_nrc_infer's kernels produce it */
+/* test hook: the encoded network input of numData DEVICE queries as gfx_nrc_infer's kernels produce it, 64 halves per query:
+ * hash grid: HashGrid 32 | OneBlob 20 | Identity 6 | ones 6 (kernel_grid grid.h:132-255, kernel_one_blob_soa oneblob.h:110-139);
+ * triangle wave: TriangleWave 36 | OneBlob 20 | Identity 6 | ones 2 (triangle_wave.h:47-81). */
 int gfx_nrc_encode_debug(gfx_nrc* nrc, void* stream, const float* inputData, uint32_t numData, void* outHalf);
 /* inference (EMA) weights as halves; gfx_nrc_set_params installs the same values as training, inference and master weights and
  * clears the optimizer state */
