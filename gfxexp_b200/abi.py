@@ -57,11 +57,6 @@ class GfxCamera(C.Structure):
     _fields_ = [("aspect", c_f), ("fovY", c_f), ("position", c_f * 3), ("orientation", c_f * 9)]
 
 
-class GfxPresentParams(C.Structure):
-    _fields_ = [("sourceBuffer", C.c_int32), ("sourceIndex", c_u32), ("mode", C.c_int32), ("flags", c_u32),
-                ("brightnessScale", c_f), ("alphaForOverride", c_f)]
-
-
 class GfxKernelTiming(C.Structure):
     _fields_ = [("label", C.c_char * 48), ("totalMs", c_f), ("launches", c_u32)]
 
@@ -85,6 +80,13 @@ class GfxFrameParams(C.Structure):
                 ("enableEnvLight", c_u32), ("envLightPowerCoeff", c_f), ("envLightRotation", c_f)]
 
 
+class GfxPresentParams(C.Structure):
+    _fields_ = [("sourceBuffer", C.c_int32), ("sourceIndex", c_u32), ("mode", C.c_int32), ("flags", c_u32),
+                ("brightnessScale", c_f), ("alphaForOverride", c_f),
+                # the debug views only (GFX_PRESENT_NRC_PREDICTION .. _FLOW, _NRC_TRAINING_PATHS, _REGIR_CELLS)
+                ("frame", C.POINTER(GfxFrameParams)), ("motionVectorScale", c_f), ("motionVectorOffset", c_f)]
+
+
 NODE_DTYPE = np.dtype([("quantBoxOrigin", np.float32, 3), ("quantBoxExpScale", np.uint8, 3),
                        ("internalMask", np.uint8), ("intNodeChildBaseIndex", np.uint32),
                        ("leafBaseIndex", np.uint32), ("childMetas", np.uint8, 8),
@@ -99,7 +101,7 @@ assert NODE_DTYPE.itemsize == 80 and TRI_DTYPE.itemsize == 48 and HIT_DTYPE.item
 
 # enums
 TRACE_CLOSEST, TRACE_ANY, TRACE_STATS = 0, 1, 2
-PT_BASELINE, PT_NRC, PT_REGIR = 0, 1, 2  # GfxPathTraceVariant
+PT_BASELINE, PT_NRC, PT_REGIR, PT_NRC_VISUALIZE_PREDICTION = 0, 1, 2, 3  # GfxPathTraceVariant
 NRC_READ_MASTER, NRC_READ_TRAINING, NRC_READ_INFERENCE, NRC_READ_GRADIENTS = 0, 1, 2, 3  # gfx_nrc_read
 NRC_POSITION_ENCODING_TRIANGLE_WAVE, NRC_POSITION_ENCODING_HASH_GRID = 0, 1  # gfx_nrc_create_with_encoding (PositionEncoding)
 (RESTIR_INITIAL_RIS, RESTIR_INITIAL_AND_TEMPORAL_BIASED, RESTIR_INITIAL_AND_TEMPORAL_UNBIASED,
@@ -117,8 +119,8 @@ SVGF_IS_FIRST_FRAME, SVGF_ENABLE_TEMPORAL_ACCUMULATION, SVGF_FEEDBACK_1ST, SVGF_
 
 # logical per-pixel layout of each downloadable buffer: (numpy dtype, elements per pixel, planes)
 BUF_PRESENT_RGBA8 = 33
-PRESENT_COLOR, PRESENT_NORMAL = 0, 1
-PRESENT_TONE_MAP, PRESENT_SRGB_GAMMA, PRESENT_FLIP_Y = 1, 2, 4
+PRESENT_COLOR, PRESENT_NORMAL, PRESENT_NRC_PREDICTION, PRESENT_NRC_PATH_LENGTH, PRESENT_FLOW = 0, 1, 2, 3, 4
+PRESENT_TONE_MAP, PRESENT_SRGB_GAMMA, PRESENT_FLIP_Y, PRESENT_NRC_TRAINING_PATHS, PRESENT_REGIR_CELLS = 1, 2, 4, 8, 16
 BUF_PEER_FLAGS = -1  # GFX_BUF_PEER_FLAGS: the flag block of the peer exchange (csrc/peer.cu)
 
 BUFFER_LAYOUT = {

@@ -279,6 +279,8 @@ int ensureRearch(gfx_ctx* ctx, uint32_t raysPerPixel);
 int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int pass, uint32_t stage);
 int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int variant);
 int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p);
+int launchNrcVisualizePrediction(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p);
+void regirGrid(const GfxFrameParams* p, uint32_t dim[3], float origin[3], float cellSize[3]); // regir.cu
 int ensurePathTraceBuffers(gfx_ctx* ctx);
 int ensureNrcFrame(gfx_ctx* ctx);
 void* ncclSymbol(const char* name); // peer.cu: NCCL entry points resolved at run time from the NCCL the host process loaded

@@ -800,6 +800,58 @@ int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* 
 }
 
 // ---------------------------------------------------------------------------------------------------------
+// visualizePrediction (optix_pathtracing_kernels.cu:702-778): the primary hit's radiance query, as k_nrcFirstHit builds it,
+// at row y * W + x; a miss leaves its row untouched
+__global__ void __launch_bounds__(64) k_nrcVisualizeQueries(DevScene s, DevFrame f, DevFrameParams p, DevNrc n) {
+    const uint32_t x = blockIdx.x * 8 + threadIdx.x;
+    const uint32_t y = blockIdx.y * 8 + threadIdx.y;
+    if (x >= f.W || y >= f.H)
+        return;
+    const uint32_t pix = y * f.W + x;
+    if (pix == 0) // what the host passes to infer() there (neural_radiance_caching_main.cpp:2376-2384)
+        n.state[NRC_NUM_INFERENCE_QUERIES] = (f.W * f.H + 127) / 128 * 128;
+    const uint4 gb0 = f.gb0[p.bufferIndex][pix];
+    const bool hit = gb0.x != 0xFFFFFFFFu;
+    if (hit) {
+        const DevInstance* inst = s.instances + gb0.x;
+        const DevMesh mesh = s.meshes[gb0.y];
+        const float bcB = decodeBarycentric((uint16_t)(gb0.w & 0xFFFFu));
+        const float bcC = decodeBarycentric((uint16_t)(gb0.w >> 16));
+        SurfacePoint sp;
+        computeSurfacePointFromGBuffer(s, inst, mesh, gb0.z, bcB, bcC, &sp);
+        f3 vOut = p.camera.position - sp.positionInWorld;
+        const float primaryDist2 = sqLength(vOut);
+        vOut /= sqrtf(primaryDist2);
+        const float primaryDotVN = dot(vOut, sp.geometricNormalInWorld);
+        const float frontHit = primaryDotVN >= 0.0f ? 1.0f : -1.0f;
+        const f3 positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
+        const ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+        const BSDF bsdf = setupBsdfAtHit(s, mesh, gb0.z, bcB, bcC);
+        createRadianceQuery(p, positionInWorld, shadingFrame.normal, vOut, bsdf, n.inferenceQuery + 14 * (size_t)pix);
+    }
+    n.terminalInfo[pix] = packTerminalInfo(f3(1.0f), 1, hit, false, false);
+}
+
+int launchNrcVisualizePrediction(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params) {
+    FrameState &F = ctx->frame;
+    if (!F.nrc.created) {
+        ctx->setError("gfx_pathtrace_launch(GFX_PT_NRC_VISUALIZE_PREDICTION): the frame has no NRC buffers yet (gfx_nrc_preprocess)");
+        return GFX_ERR_NOT_READY;
+    }
+    if (F.nrc.shardComm != nullptr && F.nrc.shardWorld > 1) {
+        ctx->setError("gfx_pathtrace_launch(GFX_PT_NRC_VISUALIZE_PREDICTION): not available on a context sharded with gfx_nrc_shard");
+        return GFX_ERR_UNSUPPORTED;
+    }
+    const DevFrameParams p = makeDevParams(ctx, params);
+    const dim3 block(8, 8), grid((F.W + 7) / 8, (F.H + 7) / 8);
+    { GFX_TIMED(ctx, stream, "nrc_visualize_queries");
+    k_nrcVisualizeQueries<<<grid, block, 0, stream>>>(ctx->devScene(params), ctx->devFrame(), p, makeDevNrc(ctx)); }
+    ctx->launches++;
+    GFX_CUDA(ctx, cudaGetLastError());
+    return GFX_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------
 // nrc_setup_kernels.cu:51-92
 __global__ void __launch_bounds__(256) k_nrcAccumulate(DevFrame f, DevFrameParams p, DevNrc n) {
     const uint32_t i = p.y0 * f.W + blockIdx.x * blockDim.x + threadIdx.x;

@@ -253,6 +253,8 @@ DevPathState makePathState(const gfx_ctx* ctx) {
 int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int variant) {
     if (variant == GFX_PT_NRC)
         return launchPathTraceNrc(ctx, stream, params);
+    if (variant == GFX_PT_NRC_VISUALIZE_PREDICTION)
+        return launchNrcVisualizePrediction(ctx, stream, params);
     if (variant != GFX_PT_BASELINE && variant != GFX_PT_REGIR) {
         ctx->setError("gfx_pathtrace_launch: unknown variant");
         return GFX_ERR_INVALID_ARGUMENT;

@@ -44,23 +44,33 @@ void releaseRegir(gfx_ctx* ctx) {
     R = FrameState::Regir();
 }
 
+// the cell grid over the scene's box (regir_main.cpp:1109, 1012)
+void regirGrid(const GfxFrameParams* p, uint32_t dim[3], float origin[3], float cellSize[3]) {
+    for (int c = 0; c < 3; ++c)
+        dim[c] = p->regirGridDim[c];
+    if (dim[0] == 0 || dim[1] == 0 || dim[2] == 0) {
+        dim[0] = 32; dim[1] = 8; dim[2] = 32;
+    }
+    for (int c = 0; c < 3; ++c) {
+        origin[c] = p->sceneAabbMin[c];
+        cellSize[c] = (p->sceneAabbMax[c] - p->sceneAabbMin[c]) / (float)dim[c];
+    }
+}
+
 // initializeReservoirs (regir_main.cpp:1073-1095)
 static int ensureRegir(gfx_ctx* ctx, const GfxFrameParams* p) {
     FrameState::Regir &R = ctx->frame.regir;
-    uint32_t dim[3] = { p->regirGridDim[0], p->regirGridDim[1], p->regirGridDim[2] };
-    if (dim[0] == 0 || dim[1] == 0 || dim[2] == 0) {
-        dim[0] = 32; dim[1] = 8; dim[2] = 32; // regir_main.cpp:1109
-    }
+    uint32_t dim[3];
+    float origin[3], cellSize[3];
+    regirGrid(p, dim, origin, cellSize);
     if (R.created && R.dim[0] == dim[0] && R.dim[1] == dim[1] && R.dim[2] == dim[2])
         return GFX_OK;
     releaseRegir(ctx);
     memcpy(R.dim, dim, sizeof(dim));
     R.numCells = dim[0] * dim[1] * dim[2];
     R.numSlots = R.numCells * kNumLightSlotsPerCell;
-    for (int c = 0; c < 3; ++c) {
-        R.gridOrigin[c] = p->sceneAabbMin[c];
-        R.gridCellSize[c] = (p->sceneAabbMax[c] - p->sceneAabbMin[c]) / (float)dim[c];
-    }
+    memcpy(R.gridOrigin, origin, sizeof(origin));
+    memcpy(R.gridCellSize, cellSize, sizeof(cellSize));
     for (int i = 0; i < 2; ++i) {
         GFX_CUDA(ctx, cudaMalloc(&R.slots[i], (size_t)R.numSlots * 64));
         GFX_CUDA(ctx, cudaMemset(R.slots[i], 0, (size_t)R.numSlots * 64));

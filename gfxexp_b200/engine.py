@@ -192,10 +192,15 @@ class Context:
 
     def present(self, source_buffer: int = abi.BUF_BEAUTY_ACCUM, source_index: int = 0, mode: int = abi.PRESENT_COLOR,
                 flags: int = abi.PRESENT_TONE_MAP | abi.PRESENT_SRGB_GAMMA, brightness_scale: float = 1.0,
-                alpha_override: float = 1.0, stream=None) -> np.ndarray:
+                alpha_override: float = 1.0, stream=None, frame_params=None, motion_vector_scale: float = 0.1,
+                motion_vector_offset: float = 0.5) -> np.ndarray:
         """accumulation buffer -> tone-mapped, sRGB-encoded RGBA8 [H, W] uint32 (R | G << 8 | B << 16 | A << 24), the
-        packing of the reference's saveImage(path, w, h, const uint32_t*)"""
-        pp = abi.GfxPresentParams(source_buffer, source_index, mode, flags, brightness_scale, alpha_override)
+        packing of the reference's saveImage(path, w, h, const uint32_t*).  The debug views (modes PRESENT_NRC_PREDICTION,
+        PRESENT_NRC_PATH_LENGTH, PRESENT_FLOW, flags PRESENT_NRC_TRAINING_PATHS, PRESENT_REGIR_CELLS) need frame_params:
+        its bufferIndex, radianceScale, scene box and ReGIR grid"""
+        pp = abi.GfxPresentParams(source_buffer, source_index, mode, flags, brightness_scale, alpha_override,
+                                  C.pointer(frame_params) if frame_params is not None else None,
+                                  motion_vector_scale, motion_vector_offset)
         self._check(self.lib.gfx_present_launch(self.h, stream, C.byref(pp)), "gfx_present_launch")
         return self.download(abi.BUF_PRESENT_RGBA8)
 
@@ -241,6 +246,13 @@ class Context:
 
     def nrc_frame_infer(self, net: "NeuralRadianceCache", stream=None):
         self._check(self.lib.gfx_nrc_frame_infer(self.h, net.h, stream), "gfx_nrc_frame_infer")
+
+    def nrc_visualize_prediction(self, net: "NeuralRadianceCache", params, stream=None):
+        """the "Directly Visualized Prediction" display (neural_radiance_caching_main.cpp:2371-2387): one radiance query
+        per primary hit of the G-buffer params.bufferIndex, then the W*H inference; show it with
+        present(mode=abi.PRESENT_NRC_PREDICTION, frame_params=params)"""
+        self.pathtrace(params, abi.PT_NRC_VISUALIZE_PREDICTION, stream)
+        self.nrc_frame_infer(net, stream)
 
     def nrc_accumulate(self, params, stream=None):
         self._check(self.lib.gfx_nrc_accumulate(self.h, stream, C.byref(params)), "gfx_nrc_accumulate")

@@ -8,10 +8,15 @@
 // types.  Scene and default parameters come from a flat binary file written by gfxexp_b200/scenes.py::save_scene_bin.
 //
 //   gfx_headless <scene.bin> <renderer> <width> <height> <frames> <out.raw> [nrc_params.f16] [-position-encoding tri|hash]
+//                [-view prediction|pathlength|flow|cells]
 //   -position-encoding: the NRC network's position encoding, as the reference app's command line takes it
 //   (neural_radiance_caching_main.cpp:458, 755-766); hash grid by default.  nrc_params.f16 must hold that network's
 //   gfx_nrc_num_params halves.
 //   renderer: restir | restir_unbiased | rearch | rearch_unbiased | pathtrace | regir | nrc
+//   -view (with a .png output): write a debug view after the last frame instead of the beauty, as the reference apps'
+//   "buffer to display" choices show it (gfx_present_launch): prediction = "Directly Visualized Prediction" (nrc: the
+//   visualizePrediction pass + inference of the primary hits, neural_radiance_caching_main.cpp:2371-2387), pathlength =
+//   "Rendering Path Length" (nrc), flow = "Motion Vector" (any renderer), cells = "Visualize Cells" (regir).
 // Output: the accumulated beauty buffer (float4 per pixel, row-major) after <frames> frames, plus one line of JSON
 // with the mean milliseconds per frame (wall clock around a synchronised loop).
 #include "gfxb200.h"
@@ -100,11 +105,12 @@ void loadScene(const char* path, uint32_t width, uint32_t height, SceneFile* s) 
 int main(int argc, char** argv) {
     if (argc < 7) {
         fprintf(stderr, "usage: %s <scene.bin> <renderer> <width> <height> <frames> <out.raw | out.png> [nrc_params.f16] "
-                "[-position-encoding tri|hash]\n", argv[0]);
+                "[-position-encoding tri|hash] [-view prediction|pathlength|flow|cells]\n", argv[0]);
         return 2;
     }
     const char* nrcParamsPath = nullptr;
     int positionEncoding = GFX_NRC_POSITION_ENCODING_HASH_GRID;
+    std::string view;
     for (int i = 7; i < argc; ++i) {
         const std::string arg = argv[i];
         if (arg == "-position-encoding" && i + 1 < argc) {
@@ -118,6 +124,13 @@ int main(int argc, char** argv) {
                 return 2;
             }
         }
+        else if (arg == "-view" && i + 1 < argc) {
+            view = argv[++i];
+            if (view != "prediction" && view != "pathlength" && view != "flow" && view != "cells") {
+                fprintf(stderr, "-view takes prediction, pathlength, flow or cells, not %s\n", view.c_str());
+                return 2;
+            }
+        }
         else if (!nrcParamsPath && arg[0] != '-')
             nrcParamsPath = argv[i];
         else {
@@ -126,6 +139,14 @@ int main(int argc, char** argv) {
         }
     }
     const std::string renderer = argv[2];
+    const std::string outPath = argv[6];
+    const bool pngOut = outPath.size() > 4 && outPath.compare(outPath.size() - 4, 4, ".png") == 0;
+    if (!view.empty() && (!pngOut || ((view == "prediction" || view == "pathlength") && renderer != "nrc") ||
+                          (view == "cells" && renderer != "regir"))) {
+        fprintf(stderr, "-view %s needs a .png output and %s\n", view.c_str(),
+                view == "cells" ? "the regir renderer" : view == "flow" ? "nothing else" : "the nrc renderer");
+        return 2;
+    }
     const uint32_t width = (uint32_t)atoi(argv[3]), height = (uint32_t)atoi(argv[4]);
     const int frames = atoi(argv[5]);
     gfx_ctx* gfx = nullptr;
@@ -243,11 +264,22 @@ int main(int argc, char** argv) {
             totalMs += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         }
 
-        const std::string outPath = argv[6];
-        if (outPath.size() > 4 && outPath.compare(outPath.size() - 4, 4, ".png") == 0) {
+        if (pngOut) {
             // the reference's screenshot: tone map + sRGB gamma on the accumulated beauty (saveImage with
             // SDRImageSaverConfig, common_host.cpp:2859-2897; brightness 0 -> scale 10^0), written as PNG
-            GfxPresentParams pp = { GFX_BUF_BEAUTY_ACCUM, 0, GFX_PRESENT_COLOR, GFX_PRESENT_TONE_MAP | GFX_PRESENT_SRGB_GAMMA, 1.0f, 1.0f };
+            GfxPresentParams pp = { GFX_BUF_BEAUTY_ACCUM, 0, GFX_PRESENT_COLOR, GFX_PRESENT_TONE_MAP | GFX_PRESENT_SRGB_GAMMA, 1.0f, 1.0f,
+                                    &fp, 0.1f, 0.5f };  // motion vectors x 10^-1 + 0.5 (neural_radiance_caching_main.cpp:2462)
+            if (view == "prediction") {                                                    // :2371-2387
+                check(gfx, gfx_pathtrace_launch(gfx, nullptr, &fp, GFX_PT_NRC_VISUALIZE_PREDICTION), "visualizePrediction");
+                check(gfx, gfx_nrc_frame_infer(gfx, nrc, nullptr), "neuralRadianceCache.infer");
+                pp.mode = GFX_PRESENT_NRC_PREDICTION;
+            }
+            else if (view == "pathlength")
+                pp.mode = GFX_PRESENT_NRC_PATH_LENGTH;
+            else if (view == "flow")
+                pp.mode = GFX_PRESENT_FLOW;
+            else if (view == "cells")
+                pp.flags |= GFX_PRESENT_REGIR_CELLS;
             check(gfx, gfx_present_launch(gfx, nullptr, &pp), "gfx_present_launch");
             std::vector<uint32_t> image((size_t)width * height);
             check(gfx, gfx_buffer_download(gfx, nullptr, GFX_BUF_PRESENT_RGBA8, 0, image.data(), image.size() * 4), "gfx_buffer_download");

@@ -270,8 +270,20 @@ typedef enum GfxPathTraceVariant {
     GFX_PT_BASELINE = 0,                        /* pathTraceBaseline */
     GFX_PT_NRC = 1,                             /* pathTraceNRC (neural_radiance_caching_main.cpp:2281-2289):
                                                  * needs gfx_nrc_preprocess first; fills the NRC buffers below */
-    GFX_PT_REGIR = 2                            /* regir's pathTraceReGIR (regir_main.cpp:2051-2057): NEE resamples the
+    GFX_PT_REGIR = 2,                           /* regir's pathTraceReGIR (regir_main.cpp:2051-2057): NEE resamples the
                                                  * cell reservoirs built by gfx_regir_build_cells */
+    GFX_PT_NRC_VISUALIZE_PREDICTION = 3         /* visualizePrediction (neural_radiance_caching/gpu_kernels/
+                                                 * optix_pathtracing_kernels.cu:702-778): for every pixel of the G-buffer
+                                                 * params->bufferIndex (the whole frame), a primary hit writes its radiance
+                                                 * query to row y * W + x of GFX_BUF_NRC_INFERENCE_QUERY (a miss leaves its row
+                                                 * as it was); every pixel's terminal info becomes alpha 1, pathLength 1,
+                                                 * hasQuery = hit, not a training pixel or unbiased tile; the state block's
+                                                 * numInferenceQueries becomes pad128(W*H), so that gfx_nrc_frame_infer infers
+                                                 * exactly those rows (:2371-2387).  Show the result with
+                                                 * GFX_PRESENT_NRC_PREDICTION.  GFX_ERR_NOT_READY before the frame has NRC
+                                                 * buffers (gfx_nrc_preprocess creates them), GFX_ERR_UNSUPPORTED on a context
+                                                 * sharded with gfx_nrc_shard(world > 1).  The next NRC frame overwrites
+                                                 * everything it writes. */
 } GfxPathTraceVariant;
 
 /* SVGF entry points (svgf/svgf_main.cpp:2127-2172) */
@@ -356,11 +368,41 @@ int gfx_timing_read(gfx_ctx* ctx, GfxKernelTiming* out, uint32_t capacity, uint3
  * common/common_host.cpp:2859-2897, is the same arithmetic on the CPU): non-finite colours -> 0,
  * lum = sRGB luminance, colour *= (1 - exp(-brightnessScale * lum)) / lum, then sRGB_gamma_s (basic_types.h:5405-5410) and
  * 8-bit packing min(uint(v * 255), 255).  The packed image is what the reference's own
- * saveImage(path, width, height, const uint32_t*) (common_host.cpp:2715) writes with stb. */
-typedef enum GfxPresentMode { GFX_PRESENT_COLOR = 0, GFX_PRESENT_NORMAL = 1 } GfxPresentMode;
+ * saveImage(path, width, height, const uint32_t*) (common_host.cpp:2715) writes with stb.
+ *
+ * The debug views of the reference's NRC and ReGIR apps (visualizeToOutputBuffer, neural_radiance_caching/gpu_kernels/
+ * copy_buffers.cu:32-130 and regir/gpu_kernels/copy_buffers.cu:62-76,95-108) are further modes and flags.  They read the
+ * frame's buffers at the pixel (after FLIP_Y), replace or tint the colour, and then go through the same alpha override, tone
+ * map, gamma and packing (the reference tints first and its display shader tone-maps afterwards):
+ *   GFX_PRESENT_NRC_PREDICTION   if the terminal info has a query: max(inferred radiance, 0), / radianceScale when that is
+ *                                > 0, x (diffuse + specular reflectance) of the query row; then x alpha, w = 1; else 0
+ *                                (copy_buffers.cu:52-67).  After GFX_PT_NRC_VISUALIZE_PREDICTION + gfx_nrc_frame_infer this
+ *                                is the cache's prediction at the primary hits.
+ *   GFX_PRESENT_NRC_PATH_LENGTH  blue -> green -> red ramp of the terminal info's pathLength, t = min((pathLength - 1) / 5, 1)
+ *                                (:96-112); meaningful after an NRC frame
+ *   GFX_PRESENT_FLOW             clamp(motionVectorScale * mv + motionVectorOffset, 0, 1) for x and y of GFX_BUF_GBUFFER1,
+ *                                z = motionVectorOffset, w = 1 (:87-94)
+ *   GFX_PRESENT_NRC_TRAINING_PATHS  flag: training pixels x (1, .25, 1, 1), other pixels of unbiased tiles x (.25, 1, .25, 1)
+ *                                (:118-127), in every mode
+ *   GFX_PRESENT_REGIR_CELLS      flag, COLOR mode only (ignored in the others): rgb x the colour of the ReGIR cell that holds
+ *                                GFX_BUF_GBUFFER2's position (FNV-1 hash of the cell index -> PCG32 -> HSVtoRGB).  The grid is
+ *                                gfx_regir_build_cells' over frame->sceneAabbMin/Max and frame->regirGridDim (0 = 32 x 8 x 32).
+ * The NRC views read GFX_BUF_NRC_TERMINAL_INFO, _INFERRED_RADIANCE and _INFERENCE_QUERY (GFX_ERR_NOT_READY before the frame
+ * has NRC buffers); the G-buffers are those of frame->bufferIndex.  The new modes do not read the source buffer.  A new mode
+ * or flag needs `frame` (GFX_ERR_INVALID_ARGUMENT without); COLOR and NORMAL without the new flags never read the fields
+ * after alphaForOverride, so callers built against the six-field struct keep working. */
+typedef enum GfxPresentMode {
+    GFX_PRESENT_COLOR = 0,
+    GFX_PRESENT_NORMAL = 1,
+    GFX_PRESENT_NRC_PREDICTION = 2,
+    GFX_PRESENT_NRC_PATH_LENGTH = 3,
+    GFX_PRESENT_FLOW = 4
+} GfxPresentMode;
 #define GFX_PRESENT_TONE_MAP 1u
 #define GFX_PRESENT_SRGB_GAMMA 2u
 #define GFX_PRESENT_FLIP_Y 4u
+#define GFX_PRESENT_NRC_TRAINING_PATHS 8u
+#define GFX_PRESENT_REGIR_CELLS 16u
 typedef struct GfxPresentParams {
     int32_t sourceBuffer;      /* a float4-per-pixel frame buffer: GFX_BUF_BEAUTY_ACCUM, _ALBEDO_ACCUM, _NORMAL_ACCUM, GFX_BUF_SVGF_FINAL ... */
     uint32_t sourceIndex;
@@ -368,6 +410,10 @@ typedef struct GfxPresentParams {
     uint32_t flags;            /* GFX_PRESENT_* */
     float brightnessScale;     /* 10^brightness of the reference UI */
     float alphaForOverride;    /* >= 0: written instead of the source alpha (SDRImageSaverConfig::alphaForOverride) */
+    /* the debug views only (see above): */
+    const GfxFrameParams* frame;  /* host: bufferIndex, radianceScale, sceneAabbMin/Max, regirGridDim */
+    float motionVectorScale;      /* 10^-1 by default (neural_radiance_caching_main.cpp:2462) */
+    float motionVectorOffset;     /* 0.5 by default */
 } GfxPresentParams;
 /* writes GFX_BUF_PRESENT_RGBA8 (read it with gfx_buffer_download or gfx_buffer_device_ptr) */
 int gfx_present_launch(gfx_ctx* ctx, void* stream, const GfxPresentParams* params);
