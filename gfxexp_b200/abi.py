@@ -367,6 +367,7 @@ _DECLS = {
     "gfx_bvh_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "gfx_bvh_import": (C.c_int, [C.c_void_p, C.c_void_p, c_u32, C.c_void_p, c_u32, C.c_void_p, c_u32]),
     "gfx_trace_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, c_u32, C.c_void_p, C.c_int]),
+    "gfx_trace_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, c_u32, C.c_void_p, C.c_int, C.c_int]),
     "gfx_trace": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, c_u32, C.c_void_p, C.c_int]),
     "gfx_light_dist_build": (C.c_int, [C.c_void_p, C.c_void_p, c_u32]),
     "gfx_framebuffer_allgather": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, c_u32, C.c_void_p]),

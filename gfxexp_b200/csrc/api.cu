@@ -261,6 +261,8 @@ int gfx_synchronize(gfx_ctx* ctx, void* stream) {
     uint32_t flag = 0;
     GFX_CUDA(ctx, cudaMemcpy(&flag, ctx->bvh.overflowFlag, 4, cudaMemcpyDeviceToHost));
     if (flag) {
+        // reported once: the next traces on this context start clean
+        GFX_CUDA(ctx, cudaMemset(ctx->bvh.overflowFlag, 0, 4));
         ctx->setError("traversal stack overflow (kStackSize too small for this BVH)");
         return GFX_ERR_CUDA;
     }
@@ -474,6 +476,8 @@ int gfx_bvh_build(gfx_ctx* ctx, void* stream, uint32_t flags) {
         return GFX_ERR_NOT_READY;
     }
     GFX_CUDA(ctx, cudaSetDevice(ctx->device));
+    // an overflow reported against the previous tree says nothing about this one
+    GFX_CUDA(ctx, cudaMemsetAsync(ctx->bvh.overflowFlag, 0, 4, (cudaStream_t)stream));
     int rc = buildBvh(ctx, (cudaStream_t)stream, flags);
     if (rc == GFX_OK)
         rc = finishBvh(ctx, (cudaStream_t)stream);
@@ -518,6 +522,7 @@ int gfx_bvh_import(gfx_ctx* ctx, const GfxBvhNode8* nodes, uint32_t numNodes, co
     GFX_CUDA(ctx, cudaSetDevice(ctx->device));
     BvhState &B = ctx->bvh;
     B.release();
+    GFX_CUDA(ctx, cudaMemset(B.overflowFlag, 0, 4));
     GFX_CUDA(ctx, cudaMalloc(&B.nodes, (size_t)max(numNodes, 1u) * 80));
     GFX_CUDA(ctx, cudaMalloc(&B.primRefs, (size_t)max(numPrimRefs, 1u) * 4));
     GFX_CUDA(ctx, cudaMalloc(&B.tris, (size_t)max(numTris, 1u) * 48));
@@ -543,6 +548,17 @@ int gfx_trace_device(gfx_ctx* ctx, void* stream, const GfxRay* rays, uint32_t nu
     if ((!rays || !hits) && numRays)
         return GFX_ERR_INVALID_ARGUMENT;
     return traceRays(ctx, (cudaStream_t)stream, rays, numRays, hits, mode);
+}
+
+int gfx_trace_debug(gfx_ctx* ctx, void* stream, const GfxRay* rays, uint32_t numRays, GfxHitObject* hits, int mode, int kernel) {
+    CHECK_CTX(ctx);
+    if (!ctx->bvh.ready) {
+        ctx->setError("gfx_trace_debug: BVH not built");
+        return GFX_ERR_NOT_READY;
+    }
+    if ((!rays || !hits) && numRays)
+        return GFX_ERR_INVALID_ARGUMENT;
+    return traceRaysDebug(ctx, (cudaStream_t)stream, rays, numRays, hits, mode, kernel);
 }
 
 int gfx_trace(gfx_ctx* ctx, void* stream, const GfxRay* rays, uint32_t numRays, GfxHitObject* hits, int mode) {

@@ -264,6 +264,8 @@ int buildBvh(gfx_ctx* ctx, cudaStream_t stream, uint32_t flags);
 int finishBvh(gfx_ctx* ctx, cudaStream_t stream);
 int launchPresent(gfx_ctx* ctx, cudaStream_t stream, const GfxPresentParams* params); // derived traversal tables of a built or imported BVH
 int traceRays(gfx_ctx* ctx, cudaStream_t stream, const GfxRay* dRays, uint32_t numRays, GfxHitObject* dHits, int mode);
+int traceRaysDebug(gfx_ctx* ctx, cudaStream_t stream, const GfxRay* dRays, uint32_t numRays, GfxHitObject* dHits, int mode,
+                   int kernel);
 int resetVisibilityQueue(gfx_ctx* ctx, cudaStream_t stream);
 int traceVisibilityQueue(gfx_ctx* ctx, cudaStream_t stream);
 int buildLightDistributions(gfx_ctx* ctx, cudaStream_t stream, uint32_t bufferIndex);

@@ -71,6 +71,54 @@ int traceRays(gfx_ctx* ctx, cudaStream_t stream, const GfxRay* dRays, uint32_t n
     return GFX_OK;
 }
 
+// One ray per thread through the fused traversal (stack in local memory), as the G-buffer kernel and the any-hit test of
+// lighting.cuh run it; gfx_trace_debug's kernel 2.
+template <bool ANY_HIT, bool STATS>
+__global__ void __launch_bounds__(128) k_traceFused(DevBvh bvh, const float4* __restrict__ rays, uint32_t numRays, HitWriter writer) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= numRays)
+        return;
+    const float4 r0 = rays[2 * (size_t)r];
+    const float4 r1 = rays[2 * (size_t)r + 1];
+    TraversalState st;
+    st.tmax = r1.w;
+    st.best = traverseBvh<ANY_HIT, STATS>(bvh, f3(r0.x, r0.y, r0.z), f3(r1.x, r1.y, r1.z), r0.w, r1.w);
+    writer.template write<ANY_HIT, STATS>(r, st);
+}
+
+int traceRaysDebug(gfx_ctx* ctx, cudaStream_t stream, const GfxRay* dRays, uint32_t numRays, GfxHitObject* dHits, int mode,
+                   int kernel) {
+    const bool anyHit = (mode & ~GFX_TRACE_STATS) == GFX_TRACE_ANY;
+    if ((mode & ~(GFX_TRACE_ANY | GFX_TRACE_STATS)) != 0 || kernel < 0 || kernel > 2 || (kernel == 1 && mode != GFX_TRACE_ANY)) {
+        ctx->setError("gfx_trace_debug: kernel 0 (wavefront), 1 (wavefront, postponed leaf tests; GFX_TRACE_ANY only) or 2 "
+                      "(fused, one ray per thread)");
+        return GFX_ERR_INVALID_ARGUMENT;
+    }
+    if (kernel == 0)
+        return traceRays(ctx, stream, dRays, numRays, dHits, mode);
+    if (numRays == 0)
+        return GFX_OK;
+    const DevScene dev = ctx->devScene();
+    const float4* r = reinterpret_cast<const float4*>(dRays);
+    HitWriter w{ dev.geomToInstMesh, reinterpret_cast<uint4*>(dHits) };
+    if (kernel == 1) {
+        uint32_t* counter = ctx->traceFetchCounter;
+        GFX_CUDA(ctx, cudaMemsetAsync(counter, 0, 4, stream));
+        const int grid = min(wavefrontGrid(), (int)((numRays + 127) / 128));
+        k_traceWavefrontDeferred<true, false><<<grid, 128, 0, stream>>>(dev.bvh, r, nullptr, numRays, counter, w);
+    } else {
+        const uint32_t grid = (numRays + 127) / 128;
+        const bool stats = (mode & GFX_TRACE_STATS) != 0;
+        if (anyHit)
+            (stats ? k_traceFused<true, true> : k_traceFused<true, false>)<<<grid, 128, 0, stream>>>(dev.bvh, r, numRays, w);
+        else
+            (stats ? k_traceFused<false, true> : k_traceFused<false, false>)<<<grid, 128, 0, stream>>>(dev.bvh, r, numRays, w);
+    }
+    ctx->launches++;
+    GFX_CUDA(ctx, cudaGetLastError());
+    return GFX_OK;
+}
+
 int resetVisibilityQueue(gfx_ctx* ctx, cudaStream_t stream) {
     GFX_CUDA(ctx, cudaMemsetAsync(ctx->frame.rayCounters, 0, 8, stream));
     return GFX_OK;

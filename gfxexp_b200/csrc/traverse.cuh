@@ -11,9 +11,11 @@
 //  * ties in hit distance resolve to the smaller TriangleStorage index instead of "first found"
 //    (makes the result independent of BVH topology, so a Morton LBVH and the reference SBVH give
 //    identical hits);
-//  * the slab test works on t = q * (scale/dir) + (origin-org)/dir with explicit FMAs and a 1e-5
-//    relative slack, i.e. it is conservative w.r.t. AABB::intersect (common/basic_types.h:3450-3465);
-//    it only decides which nodes are visited, never the hit itself.
+//  * the slab test works on t = q * (scale/dir) + (origin-org)/dir with explicit FMAs, a 1e-5 relative slack
+//    and a per-ray absolute slack that bounds the rounding error of t (derived at traverseSlack), i.e. it is
+//    conservative w.r.t. AABB::intersect (common/basic_types.h:3450-3465); it only decides which nodes are
+//    visited, never the hit itself (tests/test_traverse_host.py compiles this file for the CPU and checks that
+//    against brute force on rays aimed at edges, along axes and at the ends of the ray interval).
 //
 // The traversal is exposed as a resumable state machine (TraversalState + traverseStep = one internal
 // node incl. its leaf children) so that the wavefront kernel of trace.cu can refill finished lanes
@@ -50,6 +52,10 @@ GFX_D bool testRayVsTriangle( // common/bvh_builder.cpp:1251-1270
 
 #define GFX_CSWAP(a, b) { const uint32_t lo_ = min(a, b); const uint32_t hi_ = max(a, b); a = lo_; b = hi_; }
 
+// Relative slack of the slab test's far bound and of the culls against the closest hit so far: the distances of a box and of a
+// triangle are computed along different paths (1 / dir here, 1 / dot(normal, dir) in testRayVsTriangle).
+constexpr float kRelSlack = 1.00001f;
+
 constexpr int kStackSize = 64;
 // The wavefront kernels keep the first kSmemStack entries of every lane's stack in shared memory, laid out [entry][thread] so
 // that a warp's pushes and pops are conflict-free whatever the lanes' depths (a per-thread local-memory stack makes every push a
@@ -60,6 +66,7 @@ constexpr int kSmemStackThreads = 128; // block size of the wavefront kernels
 
 struct TraversalState {
     f3 org, dir, idir;
+    f3 slack; // per-axis absolute slack of the slab distances (traverseSlack)
     float tmin, tmax;
     Hit best;
     uint32_t nodeIdx;
@@ -105,6 +112,34 @@ GFX_D void traverseInit(TraversalState &st, const f3 &org, const f3 &dir, float 
     st.sstack = nullptr;
 }
 
+// Absolute slack s of the slab distances, per axis (u = 2^-24).  traverseStep computes a slab distance as t = fmaf(q, a, b)
+// with a = 2^e * idir (exact) and b = fl(fl(corner - org) * idir) -+ s: the distance to the exact plane corner + q 2^e of a
+// node, lowered by s for the near planes and raised by s for the far ones.  The box a builder made to contain a child,
+// though, is the decoded one, fl(corner + q 2^e) (getChildAabb; the imported reference trees rely on it).  Along one axis the
+// computed t differs from that box's plane, before the shift by s, by at most
+//   the subtraction and the product that make b       2u |b|
+//   b -+ s                                            u (|b| + s)
+//   the FMA                                           u (255 |a| + |b| + s)
+//   the decoded plane: u (|corner| + 255 2^e) away    u (|corner * idir| + 255 |a|)
+// i.e. by u (510 |a| + 4 |b| + |corner * idir| + 2s) <= 4u |idir| (255 2^e + 2 |corner| + |org|) + 2u s, as
+// |b| <= |idir| (|corner| + |org|).  Every node's box lies in the root's quantisation box [c, c + 255 2^E] and has
+// 255 2^e <= 2 * extent, so 255 2^e + 2 |corner| <= B = 2 |c| + 1024 2^E and the error is below 4u M + 2u s with
+// M = |idir| (B + |org|): s = 8u M = 2^-21 M per ray keeps every near plane in front of the decoded box's and every far plane
+// behind it, with room for the rounding of s itself and for the reference SBVH's split references, whose part boxes (clipped
+// in float) contain their part only to a fraction of an ulp of the coordinates, <= 2u |idir| |plane| <= 2u M more.
+// Without it a ray that starts near a box but far from its parent's corner (bounce and shadow rays), or meets a box far
+// from the origin, loses the box at its edges.  Per axis, so that a nearly parallel axis (huge |idir|, huge t) widens only
+// its own slab.
+GFX_D void traverseSlack(TraversalState &st, const DevBvh &bvh) {
+    const uint4 root = __ldg(bvh.nodes);
+    const f3 bound(fmaf(1024.0f, __uint_as_float((root.w & 0xFFu) << 23), 2.0f * fabsf(__uint_as_float(root.x))),
+                   fmaf(1024.0f, __uint_as_float(((root.w >> 8) & 0xFFu) << 23), 2.0f * fabsf(__uint_as_float(root.y))),
+                   fmaf(1024.0f, __uint_as_float(((root.w >> 16) & 0xFFu) << 23), 2.0f * fabsf(__uint_as_float(root.z))));
+    st.slack = f3(4.76837158e-7f * fabsf(st.idir.x) * (bound.x + fabsf(st.org.x)),
+                  4.76837158e-7f * fabsf(st.idir.y) * (bound.y + fabsf(st.org.y)),
+                  4.76837158e-7f * fabsf(st.idir.z) * (bound.z + fabsf(st.org.z)));
+}
+
 // Leaf children whose triangle tests have been postponed (wavefront kernel): the start of the triangle chain and the
 // entry distance of the leaf box.  A node step appends at most 8.
 constexpr int kPendingLeaves = 12;
@@ -147,7 +182,7 @@ GFX_D bool testLeafTriangle(const DevBvh &bvh, TraversalState &st, uint32_t idx,
 template <bool ANY_HIT, bool STATS>
 GFX_D bool testPendingTriangle(const DevBvh &bvh, TraversalState &st, PendingLeaves &pend) {
     const int top = pend.n - 1;
-    if (pend.tn[top] > st.best.dist) { // a closer hit has been found since the leaf was postponed
+    if (pend.tn[top] > st.best.dist * kRelSlack) { // a closer hit has been found since the leaf was postponed
         pend.n = top;
         return false;
     }
@@ -183,6 +218,11 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
     const float bx = (__uint_as_float(n0.x) - st.org.x) * st.idir.x;
     const float by = (__uint_as_float(n0.y) - st.org.y) * st.idir.y;
     const float bz = (__uint_as_float(n0.z) - st.org.z) * st.idir.z;
+    // near planes lowered, far planes raised by the slack (traverseSlack): the entry distance, also the one kept for the
+    // culls against the closest hit, is a lower bound, the exit distance an upper bound
+    const float bnx = bx - st.slack.x, bfx = bx + st.slack.x;
+    const float bny = by - st.slack.y, bfy = by + st.slack.y;
+    const float bnz = bz - st.slack.z, bfz = bz + st.slack.z;
 
     // The sign of the ray direction decides which quantised plane of each axis is entered first, once per node and
     // axis instead of a min/max pair per child (same t values as min(tlo, thi) / max(tlo, thi)).
@@ -200,12 +240,12 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
         const uint32_t qny = (nearY[w] >> sh) & 0xFFu, qfy = (farY[w] >> sh) & 0xFFu;
         const uint32_t qnz = (nearZ[w] >> sh) & 0xFFu, qfz = (farZ[w] >> sh) & 0xFFu;
         const bool valid = (qnx != invalidNearX) || (qfx != invalidFarX);
-        const float tnx = __fmaf_rn((float)qnx, ax, bx), tfx = __fmaf_rn((float)qfx, ax, bx);
-        const float tny = __fmaf_rn((float)qny, ay, by), tfy = __fmaf_rn((float)qfy, ay, by);
-        const float tnz = __fmaf_rn((float)qnz, az, bz), tfz = __fmaf_rn((float)qfz, az, bz);
+        const float tnx = __fmaf_rn((float)qnx, ax, bnx), tfx = __fmaf_rn((float)qfx, ax, bfx);
+        const float tny = __fmaf_rn((float)qny, ay, bny), tfy = __fmaf_rn((float)qfy, ay, bfy);
+        const float tnz = __fmaf_rn((float)qnz, az, bnz), tfz = __fmaf_rn((float)qfz, az, bfz);
         const float tn = fmaxf(fmaxf(tnx, tny), fmaxf(tnz, st.tmin));
         const float tf = fminf(fminf(tfx, tfy), fminf(tfz, st.best.dist));
-        const bool hit = valid && (tn <= tf * 1.00001f);
+        const bool hit = valid && (tn <= tf * kRelSlack);
         const uint32_t isInternal = (internalMask >> slot) & 1u;
         keys[slot] = hit ? ((isInternal << 31) | ((__float_as_uint(tn) >> 1) & 0x7FFFFFF8u) | (uint32_t)slot)
                          : 0xFFFFFFFFu;
@@ -240,7 +280,7 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
         }
         const uint32_t slot = key & 7u;
         const float tn = __uint_as_float((key & 0x7FFFFFF8u) << 1);
-        if (tn > st.best.dist)
+        if (tn > st.best.dist * kRelSlack)
             continue;
         const uint32_t metas = slot < 4 ? n1.z : n1.w;
         uint32_t idx = leafBase + ((metas >> (8 * (slot & 3))) & 0xFFu);
@@ -271,7 +311,7 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
             continue;
         const uint32_t slot = key & 7u;
         const uint32_t tnBits = (key & 0x7FFFFFF8u) << 1; // truncated entry distance (<= true tn)
-        if (__uint_as_float(tnBits) > st.best.dist)
+        if (__uint_as_float(tnBits) > st.best.dist * kRelSlack)
             continue;
         if (next != 0xFFFFFFFFu) {
             if (st.sp < kStackSize)
@@ -288,7 +328,7 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
     }
     while (st.sp > 0) {
         const uint2 e = stackLoad<SMEM_STRIDE>(st, --st.sp);
-        if (__uint_as_float(e.y) <= st.best.dist) {
+        if (__uint_as_float(e.y) <= st.best.dist * kRelSlack) {
             st.nodeIdx = e.x;
             return true;
         }
@@ -302,6 +342,7 @@ GFX_D Hit traverseBvh(const DevBvh &bvh, const f3 &org, const f3 &dir, const flo
     traverseInit(st, org, dir, tmin, tmax);
     if (bvh.numNodes == 0)
         return st.best;
+    traverseSlack(st, bvh);
     while (traverseStep<ANY_HIT, STATS>(bvh, st)) {
     }
     return st.best;
@@ -315,6 +356,7 @@ GFX_D Hit traverseBvhSmemStack(const DevBvh &bvh, const f3 &org, const f3 &dir, 
     st.sstack = sstack;
     if (bvh.numNodes == 0)
         return st.best;
+    traverseSlack(st, bvh);
     while (traverseStep<ANY_HIT, false, false, STRIDE>(bvh, st)) {
     }
     return st.best;

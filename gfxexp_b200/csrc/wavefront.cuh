@@ -65,6 +65,7 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
                     const float4 r0 = __ldg(rays + 2 * (size_t)r);
                     const float4 r1 = __ldg(rays + 2 * (size_t)r + 1);
                     traverseInit(st, f3(r0.x, r0.y, r0.z), f3(r1.x, r1.y, r1.z), r0.w, r1.w);
+                    traverseSlack(st, bvh);
                     st.sstack = myStack;
                     myRay = r;
                     active = true;
@@ -117,6 +118,7 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
                     const float4 r0 = __ldg(rays + 2 * (size_t)r);
                     const float4 r1 = __ldg(rays + 2 * (size_t)r + 1);
                     traverseInit(st, f3(r0.x, r0.y, r0.z), f3(r1.x, r1.y, r1.z), r0.w, r1.w);
+                    traverseSlack(st, bvh);
                     st.sstack = myStack;
                     myRay = r;
                     active = true;

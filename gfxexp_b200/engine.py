@@ -104,6 +104,11 @@ class Context:
     def trace_device(self, d_rays: int, num_rays: int, d_hits: int, mode: int = abi.TRACE_CLOSEST, stream=None):
         self._check(self.lib.gfx_trace_device(self.h, stream, d_rays, num_rays, d_hits, mode), "gfx_trace_device")
 
+    def trace_debug(self, d_rays: int, num_rays: int, d_hits: int, mode: int = abi.TRACE_CLOSEST, kernel: int = 0, stream=None):
+        """test hook: the records of trace_device through one traversal kernel (0 wavefront, 1 wavefront with postponed leaf
+        tests, TRACE_ANY only, 2 fused one ray per thread)"""
+        self._check(self.lib.gfx_trace_debug(self.h, stream, d_rays, num_rays, d_hits, mode, kernel), "gfx_trace_debug")
+
     def build_light_distributions(self, buffer_index: int = 0, stream=None):
         self._check(self.lib.gfx_light_dist_build(self.h, stream, buffer_index), "gfx_light_dist_build")
 

@@ -464,6 +464,12 @@ int gfx_trace_device(gfx_ctx* ctx, void* stream, const GfxRay* rays, uint32_t nu
                      GfxHitObject* hits, int mode);
 int gfx_trace(gfx_ctx* ctx, void* stream, const GfxRay* rays, uint32_t numRays,
               GfxHitObject* hits, int mode);
+/* test hook of the traversal kernels: the records and modes of gfx_trace_device (DEVICE pointers) through kernel
+ * 0 = the wavefront kernel of gfx_trace, 1 = the wavefront kernel with postponed leaf tests of the ReSTIR visibility queue
+ * (mode GFX_TRACE_ANY only), 2 = the fused traversal of the G-buffer pass and the lighting any-hit test, one ray per thread.
+ * Other kernels or modes: GFX_ERR_INVALID_ARGUMENT. */
+int gfx_trace_debug(gfx_ctx* ctx, void* stream, const GfxRay* rays, uint32_t numRays,
+                    GfxHitObject* hits, int mode, int kernel);
 
 /* replaces Scene::setupLightGeomDistributions (static part, once) and
  * Scene::setupLightInstDistribution (per frame) + ext/cubd ExclusiveSum */

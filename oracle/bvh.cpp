@@ -826,6 +826,38 @@ static inline float3 f3(const float* p) { return float3(p[0], p[1], p[2]); }
 
 enum class HitMode { FirstFound, Canonical, Any };
 
+// The slab test of the parity modes (canonical, any hit).  AABB::intersectRay (:1393) is exact about neither end: a zero
+// direction component gives 0 * inf = NaN on a box face through the origin, and the computed distances of a ray passing a box
+// edge can cross.  Per axis (u = 2^-24), t = fl(fl(plane - org) * idir) errs by u |plane - org| |idir| + u |t|, at most
+// 2u |idir| (|plane| + |org|); and the boxes themselves contain their triangles only to the precision of the coordinates: the
+// SBVH clips split references in float, so the box of a part can miss a point of the part by a fraction of an ulp
+// (<= 2u |plane|).  Together at most 4u |idir| (|plane| + |org|) per plane, a term in the size of the coordinates, not of t:
+// a ray with a short hit far from the origin needs it.  So each axis gets s = 2^-21 |idir| (|min| + |max| + |org|), twice that
+// bound, the near distances are lowered and the far ones raised by it, and the far bound is widened by 1e-5 relative for the
+// culls against the closest hit.  The reciprocal is guarded like the CUDA traverser's (components below 2^-80 become +-2^-80),
+// so a nearly parallel axis widens only its own slab.  The test decides which boxes are visited, never a hit, so a box it
+// keeps too many only costs time.
+static inline bool intersectBoxConservative(const AABB &box, const float3 &org, const float3 &idir, float distMin,
+                                            float distMax, float* hitDistMin, float* hitDistMax) {
+    float tn = distMin, tf = distMax * 1.00001f;
+    for (int a = 0; a < 3; ++a) {
+        const float t0 = (box.minP[a] - org[a]) * idir[a];
+        const float t1 = (box.maxP[a] - org[a]) * idir[a];
+        const float slack = 4.76837158e-7f * std::fabs(idir[a]) *
+                            (std::fabs(box.minP[a]) + std::fabs(box.maxP[a]) + std::fabs(org[a]));
+        tn = std::fmax(tn, std::fmin(t0, t1) - slack);
+        tf = std::fmin(tf, std::fmax(t0, t1) + slack);
+    }
+    *hitDistMin = tn;
+    *hitDistMax = tf;
+    return tn <= tf;
+}
+static inline float3 guardedReciprocal(const float3 &dir) {
+    const float ooeps = 8.271806e-25f; // 2^-80
+    auto g = [&](float d) { return 1.0f / (std::fabs(d) > ooeps ? d : std::copysign(ooeps, d)); };
+    return float3(g(dir.x), g(dir.y), g(dir.z));
+}
+
 template <HitMode mode>
 static inline HitObject traverseImpl(const GeometryBVH &bvh, const float3 &rayOrg, const float3 &rayDir,
                                      const float distMin, const float distMax, TraversalStatistics* stats) {
@@ -859,6 +891,7 @@ static inline HitObject traverseImpl(const GeometryBVH &bvh, const float3 &rayOr
     };
     Entry stack[64];
     uint8_t leafOffsets[kArity] = {};
+    const float3 invDir = guardedReciprocal(rayDir);
     int32_t stackIdx = 0;
     Entry curGroup = { 0, 0, 0, 1 };
 
@@ -899,9 +932,11 @@ static inline HitObject traverseImpl(const GeometryBVH &bvh, const float3 &rayOr
                 // The reference culls a child box against the current closest distance exactly (:1393); a triangle whose
                 // computed distance is an ulp inside a box whose computed entry is an ulp outside is then lost, and which
                 // of two near-equal hits survives depends on the tree.  The canonical / any-hit modes (the parity modes)
-                // widen the far bound by 1e-5 like the CUDA traverser, so that they equal the brute-force answer.
-                const float cullDist = mode == HitMode::FirstFound ? ret.dist : ret.dist * 1.00001f;
-                if (aabb.intersectRay(rayOrg, rayDir, distMin, cullDist, &hitDistMin, &hitDistMax)) {
+                // use the conservative test above, so that they equal the brute-force answer.
+                const bool boxHit = mode == HitMode::FirstFound
+                    ? aabb.intersectRay(rayOrg, rayDir, distMin, ret.dist, &hitDistMin, &hitDistMax)
+                    : intersectBoxConservative(aabb, rayOrg, invDir, distMin, ret.dist, &hitDistMin, &hitDistMax);
+                if (boxHit) {
                     const bool isLeaf = ((intNode.internalMask >> slot) & 1) == 0;
                     const float dist = 0.5f * (hitDistMin + hitDistMax);
                     keys[slot] = (floatToOrderedUInt(dist) >> 1) | ((isLeaf ? 0u : 1u) << 31);

@@ -130,6 +130,20 @@ def signed_zero_scene(n=SAH_HUGE_NODE + 9000, seed=5):
     return scene_of([mesh(verts, np.arange(3 * n, dtype=np.uint32).reshape(n, 3))], [inst], "signed_zero")
 
 
+CORRIDOR_HALF_WIDTH = 0.05
+
+
+def corridor_scene(n=5000):
+    """n small triangles strung along x (one at every integer x, in the plane perpendicular to it, each turned by the golden
+    angle against the previous one): built with maxLeaf 1, a ray along x meets every level of a deep tree and pushes up to
+    seven siblings per level"""
+    k = np.arange(n)
+    ang = k[:, None] * 2.39996323 + np.array([0.0, 2.1, 4.2])[None, :]
+    r = np.array([1.0, 0.6, 0.9]) * CORRIDOR_HALF_WIDTH
+    verts = np.stack([np.broadcast_to(k[:, None], (n, 3)), r * np.cos(ang), r * np.sin(ang)], axis=-1).reshape(-1, 3)
+    return scene_of([mesh(verts, np.arange(3 * n, dtype=np.uint32).reshape(n, 3))], [scenes.make_instance([0])], "corridor")
+
+
 def teapot_scene():
     return scenes.teapot_like_scene(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "teapot.obj.gz"))
 

@@ -28,6 +28,13 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, name), f"{name} declared in gfxb200.h but not exported"
 
 
+def test_trace_debug_hook():
+    """gfx_trace_debug(ctx, stream, rays, n, hits, mode, kernel): the test hook of the three traversal kernels"""
+    assert "gfx_trace_debug" in _declared_symbols()
+    restype, argtypes = abi._DECLS["gfx_trace_debug"]
+    assert restype is C.c_int and argtypes[-2:] == [C.c_int, C.c_int] and len(argtypes) == 7
+
+
 def test_pod_sizes_match_reference_layouts():
     # CompressedInternalNode_T<8> 80 B, TriangleStorage 48 B, HitObject 32 B
     # (common/common_shared.h:915-917,1025,1065-1078)

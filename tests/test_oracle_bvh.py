@@ -9,6 +9,7 @@ import pytest
 
 from gfxexp_b200 import abi, scenes
 from tests import bvh_scenes as B
+from tests import trace_rays as R
 
 
 @pytest.fixture(scope="module")
@@ -69,6 +70,23 @@ def test_any_hit_equals_brute_force(oracle, tiny):
     brute = oscene.trace(rays, oracle.TRACE_BRUTE_FORCE)
     anyhit = oscene.trace(rays, oracle.TRACE_ANY)
     assert np.array_equal(anyhit["primIndex"] != 0xFFFFFFFF, brute["primIndex"] != 0xFFFFFFFF)
+
+
+@pytest.mark.parametrize("seed", [11, 4])
+@pytest.mark.parametrize("tree", ["sbvh", "sah", "lbvh", "sah_leaf1", "lbvh_leaf1"])
+@pytest.mark.parametrize("name", list(R.SCENES))
+def test_walks_equal_brute_force_on_edge_rays(oracle, name, tree, seed):
+    """The canonical and any-hit walks (the parity modes) on the ray families of tests/trace_rays.py - edges, vertices, axis-
+    parallel directions, interval ends, the deep corridor - on the reference's SBVH and the restated GPU trees, at the rays of
+    the host-compiled traversal check (seed 11) and at another seed: closest hits equal the brute force bit for bit, any-hit
+    answers are "a brute-force hit exists in (tmin, tmax)"."""
+    flags = {"sbvh": None, "sah": 0, "lbvh": B.BVH_BUILD_FAST, "sah_leaf1": 1, "lbvh_leaf1": B.BVH_BUILD_FAST | 1}[tree]
+    o, _, fam, rays = R.gpu_style_case(oracle, name, flags, seed=seed)
+    brute = o.trace(rays, oracle.TRACE_BRUTE_FORCE)
+    wrong = R.wrong_per_family(fam, o.trace(rays, oracle.TRACE_CANONICAL), brute)
+    assert sum(wrong.values()) == 0, f"canonical: wrong rays per family {wrong} of {R.RAYS_PER_FAMILY} each"
+    wrong = R.wrong_per_family(fam, o.trace(rays, oracle.TRACE_ANY), brute, any_hit=True)
+    assert sum(wrong.values()) == 0, f"any hit: wrong rays per family {wrong} of {R.RAYS_PER_FAMILY} each"
 
 
 def test_node_codec_is_conservative(tiny):
