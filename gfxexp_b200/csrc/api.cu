@@ -28,7 +28,7 @@ void SceneState::release() {
     *this = SceneState();
 }
 void BvhState::release() {
-    cudaFree(nodes); cudaFree(primRefs); cudaFree(tris); cudaFree(leafTris); cudaFree(sceneBounds);
+    cudaFree(nodes); cudaFree(primRefs); cudaFree(tris); cudaFree(leafTris); cudaFree(travNodes); cudaFree(sceneBounds);
     uint32_t* keepFlag = overflowFlag;
     void* keepScratch = scratch;
     const size_t keepScratchBytes = scratchBytes;
@@ -152,7 +152,7 @@ DevScene gfx_ctx::devScene() const {
     d.primGuide = scene.primGuide;
     d.numInstances = scene.numInstances;
     d.rayCounter = frame.stats;
-    d.bvh.nodes = reinterpret_cast<const uint4*>(bvh.nodes);
+    d.bvh.nodes = bvh.travNodes;
     d.bvh.primRefs = bvh.primRefs;
     d.bvh.tris = bvh.tris;
     d.bvh.leafTris = bvh.leafTris;

@@ -23,6 +23,7 @@
 //                    (largest-surface-area child is opened first, like the reference's task loop
 //                    :777-800), leaves of <= maxLeaf triangles (default 2), conservative 8-bit quantisation.
 #include "scene.cuh"
+#include "traverse.cuh"
 #include "context.h"
 #include <cub/cub.cuh>
 #include <chrono>
@@ -1392,8 +1393,29 @@ __global__ void k_leafTris(uint32_t numPrimRefs, const uint32_t* __restrict__ pr
     dst[2] = t2;
 }
 
+// The nodes the traverser reads: the reference-format tree with every node's child slots in octant order (octantOrderNode;
+// thread i writes the children of node i).
+__global__ void k_travNodes(uint32_t numNodes, const uint4* __restrict__ nodes, uint4* __restrict__ travNodes) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= numNodes)
+        return;
+    octantOrderNode(nodes, i, travNodes);
+}
+
 int finishBvh(gfx_ctx* ctx, cudaStream_t stream) {
     BvhState &B = ctx->bvh;
+    if (B.numNodes > B.travNodesCapacity || !B.travNodes) {
+        cudaFree(B.travNodes);
+        B.travNodes = nullptr;
+        B.travNodesCapacity = 0;
+        GFX_CUDA(ctx, cudaMalloc(&B.travNodes, (size_t)max(B.numNodes, 1u) * 80));
+        B.travNodesCapacity = max(B.numNodes, 1u);
+    }
+    if (B.numNodes) {
+        k_travNodes<<<(B.numNodes + 127) / 128, 128, 0, stream>>>(B.numNodes, static_cast<const uint4*>(B.nodes), B.travNodes);
+        ctx->launches++;
+        GFX_CUDA(ctx, cudaGetLastError());
+    }
     if (B.numPrimRefs > B.leafTrisCapacity || !B.leafTris) {
         cudaFree(B.leafTris);
         B.leafTris = nullptr;

@@ -79,12 +79,14 @@ struct BvhState {
     uint32_t* primRefs = nullptr;
     float4* tris = nullptr;      // GfxTriangleStorage[numTris]
     float4* leafTris = nullptr;  // traversal copy: TriangleStorage per primitive reference, in leaf order (see finishBvh)
+    uint4* travNodes = nullptr;  // traversal copy of the nodes, child slots in octant order (see finishBvh)
     uint32_t* sceneBounds = nullptr;
     uint32_t* overflowFlag = nullptr;
     void* scratch = nullptr;     // build scratch arena, kept between builds (bvh_build.cu)
     size_t scratchBytes = 0;
     uint32_t builtForTris = 0;   // triangle count the output arrays are sized for
     uint32_t leafTrisCapacity = 0;
+    uint32_t travNodesCapacity = 0;
     uint32_t numNodes = 0, numPrimRefs = 0, numTris = 0, levels = 0;
     float sceneMin[3] = { 0, 0, 0 }, sceneMax[3] = { 0, 0, 0 };
     bool ready = false;

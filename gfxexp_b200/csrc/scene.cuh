@@ -77,7 +77,7 @@ static_assert(offsetof(DevInstance, normalMatrix) % 16 == 0, "the normal matrix 
 static_assert(sizeof(DevInstance) % 16 == 0, "DevInstance must stay 16-byte aligned");
 
 struct DevBvh {
-    const uint4* nodes;     // 5 x uint4 per node
+    const uint4* nodes;     // 5 x uint4 per node: the traversal copy (octantOrderNode), not the reference-format tree
     const uint32_t* primRefs;
     const float4* tris;     // 3 x float4 per triangle (reference layout, indexed by TriangleStorage index)
     const float4* leafTris; // 3 x float4 per primitive reference, leaf order; .w of the third = primRef word

@@ -40,7 +40,7 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
     TraversalState st;
     bool active = false;
     uint32_t myRay = 0;
-    if (DEFER) {
+    if constexpr (DEFER) {
     // Postponed leaves: a node step only records the leaf children it hits; the triangle tests run when at least
     // kFlushLanes lanes have some to do (or a lane's list is full, or nobody can advance otherwise).  In the immediate version
     // the node step runs with most of the 32 lanes but the triangle tests inside it with few, and they issue most of the warp
