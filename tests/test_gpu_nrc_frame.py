@@ -7,6 +7,7 @@ import numpy as np
 import pytest
 
 from gfxexp_b200 import abi, engine, scenes
+from tests import nrc_records
 
 pytestmark = pytest.mark.gpu
 
@@ -125,8 +126,21 @@ def test_nrc_frames_bit_exact(gfx_ctx, oracle, max_path_length, scene_name):
     net.close()
 
 
+def _seeded_preprocess(gfx_ctx, p, tile, offsets):
+    """the NRC preprocess of a new sequence (tile 8), or with `tile` seeded as the previous frame's tile size"""
+    if tile is not None:
+        st = gfx_ctx.download_linear(abi.BUF_NRC_STATE)
+        gfx_ctx.upload(abi.BUF_NRC_STATE, 0, nrc_records.seeded_state(st, p.bufferIndex, tile))
+    gfx_ctx.nrc_preprocess(p, offsets[0], offsets[1], tile is None)
+
+
+# 4K with 4x4 tiles has every suffix slot in use: 3840 * 2160 + 518 400 = 8 812 800 queries
+SEEDED_TILE = {(3840, 2160): 4}
+
+
 @pytest.mark.parametrize("w,h,strips", [(192, 108, [(0, 34), (34, 80), (80, 108)]),
-                                         (1920, 1080, [(0, 360), (360, 1001), (1001, 1080)])])
+                                         (1920, 1080, [(0, 360), (360, 1001), (1001, 1080)]),
+                                         (3840, 2160, [(0, 720), (720, 2002), (2002, 2160)])])
 def test_frame_inference_matches_direct_inference(gfx_ctx, w, h, strips):
     """gfx_nrc_frame_infer infers as many queries as the device-side count in the state block says (pixels + training-suffix
     slots, padded to the 128-query tile) and leaves the rows beyond it alone; its predictions are the bits gfx_nrc_infer gives
@@ -141,8 +155,9 @@ def test_frame_inference_matches_direct_inference(gfx_ctx, w, h, strips):
     net = engine.NeuralRadianceCache(gfx_ctx, 2, 1e-2)
     net.set_params(engine.random_nrc_params(net.num_params, 64 * 64 * 2 + 16 * 64, seed=19, grid_amplitude=0.1))
     p = abi.default_frame_params(scene, w, h)
+    tile = SEEDED_TILE.get((w, h))
     gfx_ctx.gbuffer(p)
-    gfx_ctx.nrc_preprocess(p, 0x2545F491, 0x9E3779B9, True)
+    _seeded_preprocess(gfx_ctx, p, tile, (0x2545F491, 0x9E3779B9))
     gfx_ctx.pathtrace(p, abi.PT_NRC)
     n, capacity = w * h, abi.nrc_query_capacity(w, h)
     sentinel = np.full((capacity, 3), 0x7FC0DEAD, dtype=np.uint32).view(np.float32)  # a NaN no kernel produces
@@ -153,6 +168,8 @@ def test_frame_inference_matches_direct_inference(gfx_ctx, w, h, strips):
     st = gfx_ctx.download_linear(abi.BUF_NRC_STATE)[:, 0]
     count, num_suffix = int(st[abi.NRC_STATE_NUM_INFERENCE_QUERIES]), int(st[abi.NRC_STATE_NUM_SUFFIX_QUERIES])
     assert count % 128 == 0 and n < count <= capacity and count == n + num_suffix, (count, num_suffix, capacity)
+    if tile is not None:
+        assert st[abi.NRC_STATE_TILE_SIZE] == tile and count == capacity == n + ((w + 3) // 4) * ((h + 3) // 4), (count, capacity)
     _same(frame[count:], sentinel[count:], "rows beyond the device-side query count")
 
     queries = torch.from_numpy(gfx_ctx.download_linear(abi.BUF_NRC_INFERENCE_QUERY)[:count]).cuda()

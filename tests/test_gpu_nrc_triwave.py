@@ -8,7 +8,7 @@ import pytest
 from gfxexp_b200 import abi, engine, scenes
 from tests import oracle_nrc_triwave as OW
 from tests.test_gpu_nrc import _queries, _rel_l2, _same_bits, _tile_queries, _train_targets
-from tests.test_gpu_nrc_frame import _compare_pathtrace, _same
+from tests.test_gpu_nrc_frame import SEEDED_TILE, _compare_pathtrace, _same, _seeded_preprocess
 
 pytestmark = pytest.mark.gpu
 TRI = abi.NRC_POSITION_ENCODING_TRIANGLE_WAVE
@@ -204,7 +204,8 @@ def test_fresh_network_is_tcnn_trainer_state(gfx_ctx):
 
 
 @pytest.mark.parametrize("w,h,strips", [(192, 108, [(0, 34), (34, 80), (80, 108)]),
-                                         (1920, 1080, [(0, 360), (360, 1001), (1001, 1080)])])
+                                         (1920, 1080, [(0, 360), (360, 1001), (1001, 1080)]),
+                                         (3840, 2160, [(0, 720), (720, 2002), (2002, 2160)])])
 def test_frame_inference_matches_direct_inference(gfx_ctx, oracle, w, h, strips):
     """gfx_nrc_frame_infer with a triangle-wave net: the device-side query count, a NaN sentinel beyond it, the bits of
     gfx_nrc_infer on the same queries; gfx_nrc_frame_infer_rows over three strips: the same bits, nothing else written"""
@@ -216,8 +217,9 @@ def test_frame_inference_matches_direct_inference(gfx_ctx, oracle, w, h, strips)
     gfx_ctx.build_light_distributions(0)
     net, _, _ = _nets(gfx_ctx, oracle, 2, 19)
     p = abi.default_frame_params(scene, w, h)
+    tile = SEEDED_TILE.get((w, h))
     gfx_ctx.gbuffer(p)
-    gfx_ctx.nrc_preprocess(p, 0x2545F491, 0x9E3779B9, True)
+    _seeded_preprocess(gfx_ctx, p, tile, (0x2545F491, 0x9E3779B9))
     gfx_ctx.pathtrace(p, abi.PT_NRC)
     n, capacity = w * h, abi.nrc_query_capacity(w, h)
     sentinel = np.full((capacity, 3), 0x7FC0DEAD, dtype=np.uint32).view(np.float32)
@@ -227,6 +229,8 @@ def test_frame_inference_matches_direct_inference(gfx_ctx, oracle, w, h, strips)
     st = gfx_ctx.download_linear(abi.BUF_NRC_STATE)[:, 0]
     count, num_suffix = int(st[abi.NRC_STATE_NUM_INFERENCE_QUERIES]), int(st[abi.NRC_STATE_NUM_SUFFIX_QUERIES])
     assert count % 128 == 0 and n < count <= capacity and count == n + num_suffix
+    if tile is not None:
+        assert st[abi.NRC_STATE_TILE_SIZE] == tile and count == capacity == n + ((w + 3) // 4) * ((h + 3) // 4), (count, capacity)
     _same(frame[count:], sentinel[count:], "rows beyond the device-side query count")
     queries = torch.from_numpy(gfx_ctx.download_linear(abi.BUF_NRC_INFERENCE_QUERY)[:count]).cuda()
     direct = torch.empty((count, 3), device="cuda")

@@ -206,24 +206,29 @@ def test_strip_partition_rejects_ragged_heights():
 NRC_W, NRC_H, NRC_FRAMES = 64, 48, 3
 
 
-def _nrc_frame(O, oframe, onet, p, frame, rows=None):
+def _nrc_frame(O, oframe, onet, p, frame, rows=None, seed_tile=None):
     """one NRC frame on the oracle (network included), on `rows` = (y0, y1) or the whole frame; the perFrameRng() draws are a
-    function of the frame index"""
+    function of the frame index.  Frame 0 starts a new sequence, or continues one whose last frame had `seed_tile`."""
     from gfxexp_b200 import abi
+    from tests import nrc_records
     rng = np.random.default_rng(500 + frame)
     offsets = [int(rng.integers(0, 2 ** 32)) for _ in range(2)]
-    n = NRC_W * NRC_H
+    w, n = oframe.W, oframe.W * oframe.H
     p.frameIndex, p.bufferIndex, p.numAccumFrames = frame, frame % 2, frame
     p.tileOriginY, p.tileRows = 0, 0
     oframe.gbuffer(p)
     if rows is not None:
         p.tileOriginY, p.tileRows = rows[0], rows[1] - rows[0]
-    oframe.nrc_preprocess(p, offsets[0], offsets[1], frame == 0)
+    seeded = frame == 0 and seed_tile is not None
+    if seeded:
+        st = oframe.linear_buffer(abi.BUF_NRC_STATE, copy=False)
+        st[:] = nrc_records.seeded_state(st, p.bufferIndex, seed_tile)
+    oframe.nrc_preprocess(p, offsets[0], offsets[1], frame == 0 and not seeded)
     oframe.pathtrace(p, abi.PT_NRC)
     q = oframe.linear_buffer(abi.BUF_NRC_INFERENCE_QUERY)
     ti = oframe.linear_buffer(abi.BUF_NRC_TERMINAL_INFO)
     suffix = oframe.linear_buffer(abi.BUF_NRC_TRAIN_SUFFIX_TERMINAL)[:, 0]
-    lo, hi = (rows[0] * NRC_W, rows[1] * NRC_W) if rows is not None else (0, n)
+    lo, hi = (rows[0] * w, rows[1] * w) if rows is not None else (0, n)
     pix = lo + np.flatnonzero((ti[lo:hi, 3] & 1).astype(bool))
     sfx = n + np.flatnonzero(((suffix >> 23) & 1).astype(bool))
     idx = np.concatenate([pix, sfx])
@@ -240,31 +245,31 @@ def _nrc_frame(O, oframe, onet, p, frame, rows=None):
     p.tileOriginY, p.tileRows = 0, 0
 
 
-def _nrc_setup():
+def _nrc_setup(scene_name="tiny_city_scene", w=NRC_W, h=NRC_H):
     from gfxexp_b200 import abi, engine, scenes
     from tests import oracle_lib as O
-    scene = scenes.tiny_city_scene()
-    oframe = O.OracleFrame(O.OracleScene(scene), NRC_W, NRC_H)
+    scene = getattr(scenes, scene_name)()
+    oframe = O.OracleFrame(O.OracleScene(scene), w, h)
     onet = O.OracleNrc(2, 1e-2)
     onet.set_params(engine.random_nrc_params(onet.num_params, onet.num_matrix_weights, grid_amplitude=0.1))
-    p = abi.default_frame_params(scene, NRC_W, NRC_H)
+    p = abi.default_frame_params(scene, w, h)
     p.maxPathLength = 4
     p.radianceScale = 2.0
     return O, oframe, onet, p
 
 
-def _worker_nrc(rank, world, port, result_path):
+def _worker_nrc(rank, world, port, result_path, scene_name, w, h, frames, seed_tile):
     sys.path.insert(0, ROOT)
     os.environ["MASTER_ADDR"] = "127.0.0.1"
     os.environ["MASTER_PORT"] = str(port)
     dist.init_process_group("gloo", rank=rank, world_size=world)
     from gfxexp_b200 import abi
-    O, oframe, onet, p = _nrc_setup()
+    O, oframe, onet, p = _nrc_setup(scene_name, w, h)
     oframe.nrc_shard(rank, world)
-    rows = (rank * NRC_H // world, (rank + 1) * NRC_H // world)
+    rows = (rank * h // world, (rank + 1) * h // world)
     out = {}
-    for f in range(NRC_FRAMES):
-        _nrc_frame(O, oframe, onet, p, f, rows)
+    for f in range(frames):
+        _nrc_frame(O, oframe, onet, p, f, rows, seed_tile)
         out[f"beauty{f}"] = oframe.buffer(abi.BUF_BEAUTY_ACCUM)[rows[0]:rows[1]].copy()
         out[f"state{f}"] = oframe.linear_buffer(abi.BUF_NRC_STATE)[:8, 0].copy()
         out[f"records{f}"] = oframe.linear_buffer(abi.BUF_NRC_TRAIN_QUERY, 0).copy()
@@ -275,23 +280,23 @@ def _worker_nrc(rank, world, port, result_path):
     dist.destroy_process_group()
 
 
-def test_nrc_strips_equal_single_process(tmp_path):
-    """the numbering of the training vertices over the ranks (one count per rank and commit round exchanged), the merge of the
-    records and the replicated training reproduce the unsharded frame bit for bit: images, counters and tile sizes, all
-    records, the trained weights of both ranks"""
+def _nrc_strips_equal_single_process(tmp_path, scene_name, w, h, frames, seed_tile=None):
+    """runs the frames sharded over two ranks and unsharded, asserts they agree and returns the unsharded state words"""
     from gfxexp_b200 import abi
     result = str(tmp_path / "nrc")
-    mp.spawn(_worker_nrc, args=(2, _free_port(), result), nprocs=2, join=True)
-    O, oframe, onet, p = _nrc_setup()
+    mp.spawn(_worker_nrc, args=(2, _free_port(), result, scene_name, w, h, frames, seed_tile), nprocs=2, join=True)
+    O, oframe, onet, p = _nrc_setup(scene_name, w, h)
     got = [np.load(result + f".{r}.npz") for r in range(2)]
-    for f in range(NRC_FRAMES):
-        _nrc_frame(O, oframe, onet, p, f)
+    states = []
+    for f in range(frames):
+        _nrc_frame(O, oframe, onet, p, f, seed_tile=seed_tile)
         st = oframe.linear_buffer(abi.BUF_NRC_STATE)[:8, 0]
+        states.append(st)
         ntrain = min(int(st[f % 2]), abi.NRC_TRAIN_BUFFER_SIZE)
         assert ntrain > 30, "vacuous: no training vertices"
         beauty = oframe.buffer(abi.BUF_BEAUTY_ACCUM)
         for r in range(2):
-            rows = slice(r * NRC_H // 2, (r + 1) * NRC_H // 2)
+            rows = slice(r * h // 2, (r + 1) * h // 2)
             assert np.array_equal(got[r][f"beauty{f}"].view(np.uint32), beauty[rows].view(np.uint32)), f"frame {f} rank {r}: image"
             assert np.array_equal(got[r][f"state{f}"], st), f"frame {f} rank {r}: counters / tile sizes"
             assert np.array_equal(got[r][f"records{f}"][:ntrain].view(np.uint32),
@@ -301,3 +306,20 @@ def test_nrc_strips_equal_single_process(tmp_path):
     want = onet.get_master()
     for r in range(2):
         assert np.array_equal(got[r]["weights"].view(np.uint32), want.view(np.uint32)), f"rank {r}: trained weights"
+    return states
+
+
+def test_nrc_strips_equal_single_process(tmp_path):
+    """the numbering of the training vertices over the ranks (one count per rank and commit round exchanged), the merge of the
+    records and the replicated training reproduce the unsharded frame bit for bit: images, counters and tile sizes, all
+    records, the trained weights of both ranks"""
+    _nrc_strips_equal_single_process(tmp_path, "tiny_city_scene", NRC_W, NRC_H, NRC_FRAMES)
+
+
+def test_nrc_strips_equal_single_process_past_the_buffer(tmp_path):
+    """the same with small_city_scene at 1920x1080 and 4x4 tiles: the ranks number their vertices past the 131 072 records, each drops its own and
+    ends those suffixes with a query, and the next frame's controller acts on the count past the buffer"""
+    from gfxexp_b200 import abi
+    states = _nrc_strips_equal_single_process(tmp_path, "small_city_scene", 1920, 1080, 2, seed_tile=4)
+    assert states[0][0] > abi.NRC_TRAIN_BUFFER_SIZE and tuple(states[0][2:4]) == (4, 4), states[0]
+    assert tuple(states[1][4:6]) == (7, 7), states[1]
