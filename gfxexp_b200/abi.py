@@ -101,14 +101,16 @@ assert NODE_DTYPE.itemsize == 80 and TRI_DTYPE.itemsize == 48 and HIT_DTYPE.item
 
 # enums
 TRACE_CLOSEST, TRACE_ANY, TRACE_STATS = 0, 1, 2
-PT_BASELINE, PT_NRC, PT_REGIR, PT_NRC_VISUALIZE_PREDICTION = 0, 1, 2, 3  # GfxPathTraceVariant
+PT_BASELINE, PT_NRC, PT_REGIR, PT_NRC_VISUALIZE_PREDICTION, PT_SVGF = 0, 1, 2, 3, 4  # GfxPathTraceVariant
 NRC_READ_MASTER, NRC_READ_TRAINING, NRC_READ_INFERENCE, NRC_READ_GRADIENTS = 0, 1, 2, 3  # gfx_nrc_read
 NRC_POSITION_ENCODING_TRIANGLE_WAVE, NRC_POSITION_ENCODING_HASH_GRID = 0, 1  # gfx_nrc_create_with_encoding (PositionEncoding)
 (RESTIR_INITIAL_RIS, RESTIR_INITIAL_AND_TEMPORAL_BIASED, RESTIR_INITIAL_AND_TEMPORAL_UNBIASED,
  RESTIR_SPATIAL_BIASED, RESTIR_SPATIAL_UNBIASED, RESTIR_SHADING, RESTIR_PRESAMPLE_LIGHTS, RESTIR_PER_PIXEL_RIS,
  RESTIR_TRACE_SHADOW_RAYS, RESTIR_SHADE_AND_RESAMPLE) = range(10)
-(SVGF_TEMPORAL_ACCUMULATE, SVGF_ESTIMATE_VARIANCE, SVGF_ATROUS, SVGF_FILL_BACKGROUND, SVGF_MODULATE_TAA) = range(5)
-SVGF_IS_FIRST_FRAME, SVGF_ENABLE_TEMPORAL_ACCUMULATION, SVGF_FEEDBACK_1ST, SVGF_ENABLE_TAA, SVGF_MODULATE_ALBEDO = 1, 2, 4, 8, 16
+(SVGF_TEMPORAL_ACCUMULATE, SVGF_ESTIMATE_VARIANCE, SVGF_ATROUS, SVGF_FILL_BACKGROUND, SVGF_MODULATE_TAA,
+ SVGF_FEEDBACK_NOISY_LIGHTING) = range(6)
+(SVGF_IS_FIRST_FRAME, SVGF_ENABLE_TEMPORAL_ACCUMULATION, SVGF_FEEDBACK_1ST, SVGF_ENABLE_TAA, SVGF_MODULATE_ALBEDO,
+ SVGF_MOLLIFY_SPECULAR) = 1, 2, 4, 8, 16, 32
 (BUF_GBUFFER0, BUF_GBUFFER1, BUF_GBUFFER2, BUF_GBUFFER3, BUF_RNG, BUF_RESERVOIR, BUF_RESERVOIR_INFO,
  BUF_BEAUTY_ACCUM, BUF_ALBEDO_ACCUM, BUF_NORMAL_ACCUM, BUF_SVGF_LIGHTING_VARIANCE, BUF_SVGF_FINAL,
  BUF_SVGF_MOMENTS, BUF_SVGF_PREV_LIGHTING, BUF_SVGF_ALBEDO, BUF_SVGF_DEPTH,

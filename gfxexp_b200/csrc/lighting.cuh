@@ -568,9 +568,11 @@ static __device__ __noinline__ float4 textureFetchRepeat(const float4* texels, u
 }
 // BSDF::setup(mat, texCoord, 0.0f) (common_device.cuh:376-385, 778-826): the material's constants, or its image textures at
 // texCoord.  The textured form is out of line (and takes the tables as plain pointers): a scene without image textures runs
-// exactly the code it ran before they existed.
-static __device__ __noinline__ BSDF setupBsdfTextured(const GfxMaterialDesc* materials, const uint4* materialTextures, const uint4* texTable,
-                                                      const float4* texPool, uint32_t matSlot, float tu, float tv) {
+// exactly the code it ran before they existed.  REGULARIZE: BSDFFlags::Regularize after the texel fetch (BSDF::setup).
+template <bool REGULARIZE>
+static __device__ __forceinline__ BSDF setupBsdfTexturedBody(const GfxMaterialDesc* materials, const uint4* materialTextures,
+                                                             const uint4* texTable, const float4* texPool, uint32_t matSlot,
+                                                             float tu, float tv) {
     const GfxMaterialDesc* m = materials + matSlot;
     const uint4 tex = __ldg(materialTextures + matSlot);
     float p0[3] = { m->p0[0], m->p0[1], m->p0[2] }, p1[3] = { m->p1[0], m->p1[1], m->p1[2] }, p2 = m->p2;
@@ -589,8 +591,17 @@ static __device__ __noinline__ BSDF setupBsdfTextured(const GfxMaterialDesc* mat
         p2 = textureFetchRepeat(texPool + d.x, d.y, d.z, tu, tv).x;
     }
     BSDF b;
-    b.setup(m->bsdfType, p0, p1, p2);
+    b.setup<REGULARIZE>(m->bsdfType, p0, p1, p2);
     return b;
+}
+static __device__ __noinline__ BSDF setupBsdfTextured(const GfxMaterialDesc* materials, const uint4* materialTextures, const uint4* texTable,
+                                                      const float4* texPool, uint32_t matSlot, float tu, float tv) {
+    return setupBsdfTexturedBody<false>(materials, materialTextures, texTable, texPool, matSlot, tu, tv);
+}
+static __device__ __noinline__ BSDF setupBsdfTexturedRegularized(const GfxMaterialDesc* materials, const uint4* materialTextures,
+                                                                 const uint4* texTable, const float4* texPool, uint32_t matSlot,
+                                                                 float tu, float tv) {
+    return setupBsdfTexturedBody<true>(materials, materialTextures, texTable, texPool, matSlot, tu, tv);
 }
 GFX_D BSDF setupBsdf(const DevScene &s, uint32_t matSlot, const f2 &texCoord) {
     if (s.materialTextures)

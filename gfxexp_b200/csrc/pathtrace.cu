@@ -250,11 +250,211 @@ DevPathState makePathState(const gfx_ctx* ctx) {
     return ps;
 }
 
+// ---- the SVGF app's path tracer (GFX_PT_SVGF) ----------------------------------------------------------------
+// svgf/gpu_kernels/optix_pathtracing_kernels.cu:193-337 up to the temporal accumulation, which GFX_SVGF_TEMPORAL_ACCUMULATE
+// runs.  The first vertex is the raster G-buffer's: position, interpolated and normalised shading normal, texture
+// coordinate.  The geometric normal is that shading normal (:237), the frame is ReferenceFrame(normal) (no texture-coordinate
+// tangent) and the origin is offset naively (:242).  Miss pixels return at once (:213-219): no RNG draw, no environment.
+__global__ void GFX_BOUNCE_BOUNDS k_ptSvgfFirstHit(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps) {
+    const uint32_t x = blockIdx.x * 8 + threadIdx.x;
+    const uint32_t y = p.y0 + blockIdx.y * 8 + threadIdx.y;
+    const uint32_t lane = (threadIdx.x + threadIdx.y * blockDim.x) & 31u;
+    const bool inside = x < f.W && y < p.y1;
+    const uint32_t pix = inside ? y * f.W + x : 0u;
+
+    bool alive = false;
+    f3 positionInWorld(0.0f);
+    VertexOutput v;
+    v.wantShadow = v.wantExtension = false;
+    if (inside) {
+        const uint4 gb0 = f.gb0[p.bufferIndex][pix];
+        f3 radiance(0.0f);
+        float4 albedo = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+        if (gb0.x != 0xFFFFFFFFu) {
+            const DevInstance* inst = s.instances + gb0.x;
+            const DevMesh mesh = s.meshes[gb0.y];
+            const float bcB = decodeBarycentric((uint16_t)(gb0.w & 0xFFFFu));
+            const float bcC = decodeBarycentric((uint16_t)(gb0.w >> 16));
+            SurfacePoint sp;
+            computeSurfacePointFromGBuffer(s, inst, mesh, gb0.z, bcB, bcC, &sp);
+
+            const f3 alpha(1.0f);
+            PCG32RNG rng{ f.rng[pix] };
+            const GfxMaterialDesc* mat = s.materials + mesh.materialSlot;
+            const f3 shadingNormalInWorld = sp.shadingNormalInWorld;
+            const f3 vOut = normalize(p.camera.position - sp.positionInWorld);
+            const float frontHit = dot(vOut, shadingNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
+            const ReferenceFrame shadingFrame(shadingNormalInWorld);
+            positionInWorld = offsetRayOriginNaive(sp.positionInWorld, frontHit * shadingNormalInWorld);
+            const f3 vOutLocal = shadingFrame.toLocal(vOut);
+
+            if (vOutLocal.z > 0 && mat->hasEmittance)
+                radiance += alpha * f3(mat->emittance[0], mat->emittance[1], mat->emittance[2]) / kPi;
+            const BSDF bsdf = setupBsdfAtHit(s, mesh, gb0.z, bcB, bcC);
+            const f3 dhReflectance = bsdf.evaluateDHReflectanceEstimate(vOutLocal); // :256; the 0.001 threshold is the temporal pass's
+            albedo = make_float4(dhReflectance.x, dhReflectance.y, dhReflectance.z, 1.0f);
+            shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, &radiance, &v);
+            f.rng[pix] = rng.state;
+            ps.alphaPdf[pix] = make_float4(v.alpha.x, v.alpha.y, v.alpha.z, v.dirPDensity);
+            alive = true;
+        }
+        ps.radiance[pix] = make_float4(radiance.x, radiance.y, radiance.z, 0.0f);
+        f.albedo[pix] = albedo;
+    }
+    emitRays(s, ps, ps.counters, 0u, lane, pix, positionInWorld, v, alive);
+}
+
+// The SVGF app's closest-hit program (:381-468) and miss program (:482-513) on the compacted queue, as k_ptBounce without ReGIR:
+// no Russian roulette at pathLength 2 (round 0), whose random number is still drawn (:438-441), and with MOLLIFY the BSDF
+// set up with BSDFFlags::Regularize (:446-450).  A kernel of its own, so that k_ptBounce's code stays as it is.
+template <bool MOLLIFY>
+__global__ void GFX_BOUNCE_BOUNDS k_ptSvgfBounce(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, uint32_t round,
+                                                 uint32_t maxLengthTerminate) {
+    const uint32_t curQueue = round & 1u, nextQueue = curQueue ^ 1u;
+    const uint32_t* roundCounters = ps.counters + 4 * round;
+    uint32_t* nextCounters = ps.counters + 4 * (round + 1);
+    const uint32_t count = roundCounters[0];
+    const uint32_t lane = threadIdx.x & 31u;
+    const uint32_t warpsPerGrid = gridDim.x * (blockDim.x >> 5);
+    const uint32_t warp = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const float initImportance = sRGB_calcLuminance(f3(1.0f));
+
+    for (uint32_t base = warp * 32u; base < count; base += warpsPerGrid * 32u) {
+        const uint32_t slot = base + lane;
+        bool alive = false;
+        uint32_t pix = 0;
+        f3 positionInWorld(0.0f);
+        VertexOutput v;
+        v.wantShadow = v.wantExtension = false;
+        if (slot < count) {
+            const uint4 hit = ps.extHits[slot];
+            if (hit.y != 0xFFFFFFFFu) { // miss program: no environment light, the path ends
+                pix = ps.extPixel[curQueue][slot];
+                const float4 r0 = ps.extRays[curQueue][2 * (size_t)slot];
+                const float4 r1 = ps.extRays[curQueue][2 * (size_t)slot + 1];
+                const f3 rayOrigin(r0.x, r0.y, r0.z), rayDir(r1.x, r1.y, r1.z);
+                const float4 ap = ps.alphaPdf[pix];
+                f3 alpha(ap.x, ap.y, ap.z);
+                const float prevDirPDensity = ap.w;
+                const float4 rad = ps.radiance[pix];
+                f3 radiance(rad.x, rad.y, rad.z);
+                PCG32RNG rng{ f.rng[pix] };
+
+                const uint2 im = __ldg(s.geomToInstMesh + hit.x);
+                const DevInstance* inst = s.instances + im.x;
+                const DevMesh mesh = s.meshes[im.y];
+                SurfacePoint sp;
+                computeSurfacePointAtHit(s, inst, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), &sp);
+                const GfxMaterialDesc* mat = s.materials + mesh.materialSlot;
+
+                const f3 vOut = normalize(-rayDir);
+                const float frontHit = dot(vOut, sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
+                const ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+                positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
+                const f3 vOutLocal = shadingFrame.toLocal(vOut);
+
+                // implicit light sampling, MIS against the hypothetical NEE density (:422-435)
+                if (vOutLocal.z > 0 && mat->hasEmittance) {
+                    const f3 emittance(mat->emittance[0], mat->emittance[1], mat->emittance[2]);
+                    const float dist2 = sqLength(positionInWorld - rayOrigin);
+                    const float lightPDensity = sp.hypAreaPDensity * dist2 / vOutLocal.z;
+                    const float bsdfPDensity = prevDirPDensity;
+                    const float misWeight = pow2f(bsdfPDensity) / (pow2f(bsdfPDensity) + pow2f(lightPDensity));
+                    radiance += alpha * emittance * (misWeight / kPi);
+                }
+
+                // Russian roulette (:437-444)
+                const float continueProb = round == 0 ? 1.0f : fminf(sRGB_calcLuminance(alpha) / initImportance, 1.0f);
+                if (!(rng.getFloat0cTo1o() >= continueProb || maxLengthTerminate)) {
+                    alpha /= continueProb;
+                    const BSDF bsdf = setupBsdfAtHit<MOLLIFY>(s, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w));
+                    shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, &radiance, &v);
+                    ps.alphaPdf[pix] = make_float4(v.alpha.x, v.alpha.y, v.alpha.z, v.dirPDensity);
+                    alive = true;
+                }
+                f.rng[pix] = rng.state;
+                ps.radiance[pix] = make_float4(radiance.x, radiance.y, radiance.z, 0.0f);
+            }
+            else if (s.env.enabled) { // miss program (:482-513)
+                const uint32_t missPix = ps.extPixel[curQueue][slot];
+                const float4 r1 = ps.extRays[curQueue][2 * (size_t)slot + 1];
+                const float4 ap = ps.alphaPdf[missPix];
+                const f3 implicit = evaluateEnvLightOnMiss(s, f3(r1.x, r1.y, r1.z), ap.w, false);
+                float4 rad = ps.radiance[missPix];
+                const f3 add = f3(ap.x, ap.y, ap.z) * implicit;
+                rad.x += add.x; rad.y += add.y; rad.z += add.z;
+                ps.radiance[missPix] = rad;
+            }
+        }
+        emitRays(s, ps, nextCounters, nextQueue, lane, pix, positionInWorld, v, alive);
+    }
+}
+
+// :318-319: contribution = max(contribution, RGB(0.0f)), component-wise std::fmax: a NaN component becomes 0.  The single-spp
+// result goes to the beauty buffer as it is (no running mean: the temporal pass accumulates).
+__global__ void __launch_bounds__(256) k_ptSvgfEpilogue(DevFrame f, DevFrameParams p, DevPathState ps) {
+    const uint32_t n = (p.y1 - p.y0) * f.W;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    const size_t pix = (size_t)p.y0 * f.W + i;
+    const float4 rad = ps.radiance[pix];
+    f.beauty[pix] = make_float4(rad.x > 0.0f ? rad.x : 0.0f, rad.y > 0.0f ? rad.y : 0.0f, rad.z > 0.0f ? rad.z : 0.0f, 1.0f);
+}
+
+static int launchPathTraceSvgf(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params) {
+    const int rc = ensurePathTraceBuffers(ctx);
+    if (rc != GFX_OK)
+        return rc;
+    FrameState &F = ctx->frame;
+    DevFrameParams p = makeDevParams(ctx, params);
+    if (p.y1 <= p.y0)
+        return GFX_OK;
+    p.maxPathLength = params->maxPathLength ? params->maxPathLength : 5u; // svgf_main.cpp:1729
+    const bool mollify = (params->svgfFlags & GFX_SVGF_MOLLIFY_SPECULAR) != 0;
+    const DevScene s = ctx->devScene(params);
+    const DevFrame f = ctx->devFrame();
+    const DevPathState ps = makePathState(ctx);
+
+    const uint32_t maxPathLength = p.maxPathLength;
+    const uint32_t numRounds = min(max(maxPathLength, 2u) - 1u, kMaxPathRounds); // pathLength = 2 .. maxPathLength
+    GFX_CUDA(ctx, cudaMemsetAsync(F.ptCounters, 0, (kMaxPathRounds + 1) * 16, stream));
+
+    const dim3 block(8, 8);
+    const dim3 grid((F.W + 7) / 8, (p.y1 - p.y0 + 7) / 8);
+    { GFX_TIMED(ctx, stream, "pt_svgf_first_hit"); k_ptSvgfFirstHit<<<grid, block, 0, stream>>>(s, f, p, ps); }
+    ctx->launches++;
+    const int traceGrid = wavefrontGrid();
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
+    const ShadowAccumulateWriter shadowWriter{ ps.shadowPixel, ps.shadowPending, ps.radiance };
+    const ExtensionHitWriter extWriter{ ps.extHits };
+    for (uint32_t round = 0; round < numRounds; ++round) {
+        uint32_t* c = F.ptCounters + 4 * round;
+        { GFX_TIMED(ctx, stream, "pt_trace_shadow"); k_traceWavefront<true, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.shadowRays, c + 2, 0u, c + 3, shadowWriter); }
+        { GFX_TIMED(ctx, stream, "pt_trace_extension"); k_traceWavefront<false, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.extRays[round & 1], c + 0, 0u, c + 1, extWriter); }
+        const uint32_t maxLengthTerminate = (round + 2 >= maxPathLength || round + 1 == numRounds) ? 1u : 0u;
+        GFX_TIMED(ctx, stream, "pt_svgf_bounce");
+        if (mollify)
+            k_ptSvgfBounce<true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, round, maxLengthTerminate);
+        else
+            k_ptSvgfBounce<false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, round, maxLengthTerminate);
+        ctx->launches += 3;
+    }
+    const uint32_t numPixels = (p.y1 - p.y0) * F.W;
+    { GFX_TIMED(ctx, stream, "pt_svgf_epilogue"); k_ptSvgfEpilogue<<<(numPixels + 255) / 256, 256, 0, stream>>>(f, p, ps); }
+    ctx->launches++;
+    GFX_CUDA(ctx, cudaGetLastError());
+    return GFX_OK;
+}
+
 int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int variant) {
     if (variant == GFX_PT_NRC)
         return launchPathTraceNrc(ctx, stream, params);
     if (variant == GFX_PT_NRC_VISUALIZE_PREDICTION)
         return launchNrcVisualizePrediction(ctx, stream, params);
+    if (variant == GFX_PT_SVGF)
+        return launchPathTraceSvgf(ctx, stream, params);
     if (variant != GFX_PT_BASELINE && variant != GFX_PT_REGIR) {
         ctx->setError("gfx_pathtrace_launch: unknown variant");
         return GFX_ERR_INVALID_ARGUMENT;

@@ -50,26 +50,49 @@ GFX_D TriangleVertices fetchTriangle(const DevScene &s, const DevMesh &mesh, uin
 }
 
 // the BSDF at a hit of the path tracers (bsdf.setup(mat, texCoord, 0.0f), optix_pathtracing_kernels.cu:120-121, 283-284): the
-// texture coordinate bcA tcA + bcB tcB + bcC tcC (path_tracing_shared.h:497, 601) is only interpolated in a textured scene, out of line
-static __device__ __noinline__ BSDF setupBsdfTexturedAtHit(const GfxMaterialDesc* materials, const uint4* materialTextures, const uint4* texTable,
-                                                           const float4* texPool, const uint4* triangles, const float4* vertices,
-                                                           uint32_t triBase, uint32_t vertexBase, uint32_t matSlot, uint32_t primIndex,
-                                                           float bcB, float bcC) {
+// texture coordinate bcA tcA + bcB tcB + bcC tcC (path_tracing_shared.h:497, 601) is only interpolated in a textured scene, out of line.
+// REGULARIZE: the SVGF app's bounces, bsdf.setup(mat, texCoord, 0.0f, BSDFFlags::Regularize) (svgf optix_pathtracing_kernels.cu:448-450)
+template <bool REGULARIZE>
+static __device__ __forceinline__ BSDF setupBsdfTexturedAtHitBody(const GfxMaterialDesc* materials, const uint4* materialTextures,
+                                                                  const uint4* texTable, const float4* texPool, const uint4* triangles,
+                                                                  const float4* vertices, uint32_t triBase, uint32_t vertexBase,
+                                                                  uint32_t matSlot, uint32_t primIndex, float bcB, float bcC) {
     const uint4 tri = __ldg(triangles + triBase + primIndex);
     const float4* vA = vertices + 3 * (size_t)(vertexBase + tri.x);
     const float4* vB = vertices + 3 * (size_t)(vertexBase + tri.y);
     const float4* vC = vertices + 3 * (size_t)(vertexBase + tri.z);
     const float bcA = 1 - (bcB + bcC);
     const f2 texCoord = bcA * f2(__ldg(vA).w, __ldg(vA + 1).w) + bcB * f2(__ldg(vB).w, __ldg(vB + 1).w) + bcC * f2(__ldg(vC).w, __ldg(vC + 1).w);
+    if (REGULARIZE)
+        return setupBsdfTexturedRegularized(materials, materialTextures, texTable, texPool, matSlot, texCoord.x, texCoord.y);
     return setupBsdfTextured(materials, materialTextures, texTable, texPool, matSlot, texCoord.x, texCoord.y);
 }
+static __device__ __noinline__ BSDF setupBsdfTexturedAtHit(const GfxMaterialDesc* materials, const uint4* materialTextures, const uint4* texTable,
+                                                           const float4* texPool, const uint4* triangles, const float4* vertices,
+                                                           uint32_t triBase, uint32_t vertexBase, uint32_t matSlot, uint32_t primIndex,
+                                                           float bcB, float bcC) {
+    return setupBsdfTexturedAtHitBody<false>(materials, materialTextures, texTable, texPool, triangles, vertices, triBase, vertexBase,
+                                             matSlot, primIndex, bcB, bcC);
+}
+static __device__ __noinline__ BSDF setupBsdfTexturedAtHitRegularized(const GfxMaterialDesc* materials, const uint4* materialTextures,
+                                                                      const uint4* texTable, const float4* texPool, const uint4* triangles,
+                                                                      const float4* vertices, uint32_t triBase, uint32_t vertexBase,
+                                                                      uint32_t matSlot, uint32_t primIndex, float bcB, float bcC) {
+    return setupBsdfTexturedAtHitBody<true>(materials, materialTextures, texTable, texPool, triangles, vertices, triBase, vertexBase,
+                                            matSlot, primIndex, bcB, bcC);
+}
+template <bool REGULARIZE = false>
 GFX_D BSDF setupBsdfAtHit(const DevScene &s, const DevMesh &mesh, uint32_t primIndex, float bcB, float bcC) {
-    if (s.materialTextures)
+    if (s.materialTextures) {
+        if (REGULARIZE)
+            return setupBsdfTexturedAtHitRegularized(s.materials, s.materialTextures, s.texTable, s.texPool, s.triangles, s.vertices,
+                                                     mesh.triBase, mesh.vertexBase, mesh.materialSlot, primIndex, bcB, bcC);
         return setupBsdfTexturedAtHit(s.materials, s.materialTextures, s.texTable, s.texPool, s.triangles, s.vertices, mesh.triBase,
                                       mesh.vertexBase, mesh.materialSlot, primIndex, bcB, bcC);
+    }
     const GfxMaterialDesc* m = s.materials + mesh.materialSlot;
     BSDF b;
-    b.setup(m->bsdfType, m->p0, m->p1, m->p2);
+    b.setup<REGULARIZE>(m->bsdfType, m->p0, m->p1, m->p2);
     return b;
 }
 

@@ -161,9 +161,17 @@ GFX_D f3 offsetRayOrigin(const f3 &p, const f3 &geometricNormal) { // :114-143
                   fabsf(p.z) < kOrigin ? newP2.z : newP1.z);
 }
 
+constexpr float kRayEpsilon = 1e-4f; // RayEpsilon (:6)
+GFX_D f3 offsetRayOriginNaive(const f3 &p, const f3 &geometricNormal) { // :104-108
+    return p + kRayEpsilon * geometricNormal;
+}
+
 struct ReferenceFrame { // :151-176
     f3 tangent, bitangent, normal;
     GFX_D ReferenceFrame() {}
+    GFX_D explicit ReferenceFrame(const f3 &_normal) : normal(_normal) { // :158-160, no texture-coordinate tangent
+        makeCoordinateSystem(normal, &tangent, &bitangent);
+    }
     GFX_D ReferenceFrame(const f3 &_normal, const f3 &_tangent) : tangent(_tangent), normal(_normal) {
         bitangent = cross(normal, tangent);
     }
@@ -213,7 +221,10 @@ struct BSDF {
     f3 specularF0Color;
     float roughness;
 
-    // setupBSDFBody<...> (common_device.cuh:376-385, 778-826) with 1x1 textures
+    // setupBSDFBody<...> (common_device.cuh:376-385, 778-826) with 1x1 textures.  REGULARIZE = BSDFFlags::Regularize
+    // (:795-797, :821-823), the SVGF app's specular mollification: the smoothness is halved, for DiffuseAndSpecular before
+    // the 0.999 clamp, for SimplePBR after it; Lambert ignores the flag.
+    template <bool REGULARIZE = false>
     GFX_D void setup(uint32_t bsdfType, const float* p0, const float* p1, float p2) {
         if (bsdfType == 0) {
             type = 0;
@@ -223,7 +234,7 @@ struct BSDF {
         }
         else if (bsdfType == 1) {
             type = 1;
-            const float smoothness = fminf(p2, 0.999f);
+            const float smoothness = fminf(REGULARIZE ? p2 * 0.5f : p2, 0.999f);
             diffuseColor = f3(p0[0], p0[1], p0[2]);
             specularF0Color = f3(p1[0], p1[1], p1[2]);
             roughness = 1 - smoothness;
@@ -231,7 +242,9 @@ struct BSDF {
         else { // SimplePBR_BRDF(baseColor, 0.5f, smoothness, metallic) :767-776, :806-826
             type = 1;
             const f3 baseColor(p0[0], p0[1], p0[2]);
-            const float smoothness = fminf(1.0f - p1[1], 0.999f);
+            float smoothness = fminf(1.0f - p1[1], 0.999f);
+            if (REGULARIZE)
+                smoothness *= 0.5f;
             const float metallic = p1[2];
             const float reflectance = 0.5f;
             diffuseColor = baseColor * (1 - metallic);

@@ -2,7 +2,8 @@
 //
 // Replaces the PURE_CUDA kernels of svgf/gpu_kernels/svgf.cu (estimateVariance :30-134,
 // applyATrousFilter_box3x3 :221-354, fillBackground :378-461,
-// applyAlbedoModulationAndTemporalAntiAliasing :533-611; launch sites svgf/svgf_main.cpp:2127-2172)
+// applyAlbedoModulationAndTemporalAntiAliasing :533-611, feedbackNoisyLighting :356-374; launch sites
+// svgf/svgf_main.cpp:2127-2172)
 // and the temporal-accumulation epilogue of the SVGF path tracer
 // (svgf/gpu_kernels/optix_pathtracing_kernels.cu:12-128 reprojectPreviousAccumulation, :325-378
 // demodulation + EMA + moments).  Config 4 runs them on restir_di's output: the inputs are this
@@ -439,6 +440,13 @@ __global__ void __launch_bounds__(256) k_svgfModulateTAA(DevSvgf s, DevFramePara
     s.finalLighting[curBufIdx][pix] = make_float4(finalLighting.x, finalLighting.y, finalLighting.z, 1.0f);
 }
 
+// ---- feedbackNoisyLighting (svgf.cu:356-374) ----------------------------------------------
+// With SVGF off and temporal accumulation on, the next frame's reprojection reads the unfiltered lighting of this one.
+__global__ void __launch_bounds__(256) k_svgfFeedbackNoisyLighting(DevSvgf s, DevFrameParams p) {
+    SVGF_PIXEL();
+    s.prevLighting[pix] = s.lighting[0][pix];
+}
+
 int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int pass, uint32_t stage) {
     const DevFrameParams p = makeDevParams(ctx, params);
     if (p.y1 <= p.y0)
@@ -485,6 +493,7 @@ int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, 
         break;
     case GFX_SVGF_FILL_BACKGROUND: { GFX_TIMED(ctx, stream, "svgf_background"); k_svgfBackground<<<grid, block, 0, stream>>>(s, p, stage, ctx->devScene(params).env); } break;
     case GFX_SVGF_MODULATE_TAA: { GFX_TIMED(ctx, stream, "svgf_modulate_taa"); k_svgfModulateTAA<<<grid, block, 0, stream>>>(s, p, stage); } break;
+    case GFX_SVGF_FEEDBACK_NOISY_LIGHTING: { GFX_TIMED(ctx, stream, "svgf_feedback_noisy_lighting"); k_svgfFeedbackNoisyLighting<<<grid, block, 0, stream>>>(s, p); } break;
     default:
         ctx->setError("gfx_svgf_launch: unknown pass");
         return GFX_ERR_INVALID_ARGUMENT;

@@ -466,6 +466,54 @@ def svgf_frame_passes(params, frame_index: int, num_filtering_stages: int = 5):
     yield (abi.SVGF_MODULATE_TAA, num_filtering_stages)
 
 
+def svgf_app_frame_passes(params, frame_index: int, enable_svgf: bool = True, temporal_accumulation: bool = True,
+                          mollify: bool = True, num_filtering_stages: int = 5):
+    """The launch list of one frame of the SVGF app (svgf/svgf_main.cpp:1980-2172): light distributions, G-buffer, the app's
+    own path tracer (GFX_PT_SVGF), temporal accumulation, then variance + num_filtering_stages a-trous stages with SVGF on,
+    or feedbackNoisyLighting with SVGF off and temporal accumulation on, and last background fill + albedo modulation / TAA,
+    which read lighting plane (num_filtering_stages if SVGF is on else 0) % 2.  Yields (kind, pass_id, stage) with kind
+    "light_dist" (pass_id = buffer index), "gbuffer", "pathtrace" (pass_id = abi.PT_SVGF) or "svgf"; sets frameIndex,
+    bufferIndex, the svgfFlags of the app's switches (isFirstFrame, enableTemporalAccumulation, mollifySpecular) and
+    resetFlowBuffer (the G-buffer's motion vectors, which the reprojections read, are zero on a new sequence only) in `params`
+    as the host does."""
+    params.frameIndex = frame_index
+    params.bufferIndex = frame_index % 2
+    params.resetFlowBuffer = 1 if frame_index == 0 else 0
+    flags = params.svgfFlags & ~(abi.SVGF_IS_FIRST_FRAME | abi.SVGF_ENABLE_TEMPORAL_ACCUMULATION | abi.SVGF_MOLLIFY_SPECULAR)
+    if frame_index == 0:
+        flags |= abi.SVGF_IS_FIRST_FRAME
+    if temporal_accumulation:
+        flags |= abi.SVGF_ENABLE_TEMPORAL_ACCUMULATION
+    if mollify:
+        flags |= abi.SVGF_MOLLIFY_SPECULAR
+    params.svgfFlags = flags
+    yield ("light_dist", frame_index % 2, 0)
+    yield ("gbuffer", -1, 0)
+    yield ("pathtrace", abi.PT_SVGF, 0)
+    yield ("svgf", abi.SVGF_TEMPORAL_ACCUMULATE, 0)
+    stages = num_filtering_stages if enable_svgf else 0
+    if enable_svgf:
+        yield ("svgf", abi.SVGF_ESTIMATE_VARIANCE, 0)
+        for stage in range(num_filtering_stages):
+            yield ("svgf", abi.SVGF_ATROUS, stage)
+    elif temporal_accumulation:
+        yield ("svgf", abi.SVGF_FEEDBACK_NOISY_LIGHTING, 0)
+    yield ("svgf", abi.SVGF_FILL_BACKGROUND, stages)
+    yield ("svgf", abi.SVGF_MODULATE_TAA, stages)
+
+
+def run_svgf_app_pass(ctx: Context, params, kind: str, pass_id: int, stage: int, stream=None):
+    """issue one launch of svgf_app_frame_passes on a Context"""
+    if kind == "light_dist":
+        ctx.build_light_distributions(pass_id, stream)
+    elif kind == "gbuffer":
+        ctx.gbuffer(params, stream)
+    elif kind == "pathtrace":
+        ctx.pathtrace(params, pass_id, stream)
+    else:
+        ctx.svgf(params, pass_id, stage, stream)
+
+
 class ReSTIRRenderer:
     """Config-2 style frame driver (OriginalReSTIRBiased by default)."""
 

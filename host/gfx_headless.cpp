@@ -1,7 +1,7 @@
 // gfx_headless.cpp — a headless C++ host on top of the C ABI of include/gfxb200.h.
 //
 // The reference hosts are C++ programs (restir_di/restir_di_main.cpp, path_tracing/path_tracing_main.cpp,
-// regir/regir_main.cpp, neural_radiance_caching/neural_radiance_caching_main.cpp) whose frame loops end in OptiX /
+// regir/regir_main.cpp, neural_radiance_caching/neural_radiance_caching_main.cpp, svgf/svgf_main.cpp) whose frame loops end in OptiX /
 // CUDA launches.  This file is those frame loops with the window, UI and asset import removed and every launch line
 // replaced by the gfx_* call that INTEGRATION.md names for it; it exists to show (and to test, see
 // tests/test_gpu_host_cpp.py) that the boundary is a plain C ABI: nothing here knows about Python, torch or CUDA
@@ -12,12 +12,15 @@
 //   -position-encoding: the NRC network's position encoding, as the reference app's command line takes it
 //   (neural_radiance_caching_main.cpp:458, 755-766); hash grid by default.  nrc_params.f16 must hold that network's
 //   gfx_nrc_num_params halves.
-//   renderer: restir | restir_unbiased | rearch | rearch_unbiased | pathtrace | regir | nrc
+//   renderer: restir | restir_unbiased | rearch | rearch_unbiased | pathtrace | regir | nrc | svgf
+//   svgf: the SVGF app's frame (svgf_main.cpp:1980-2172) with its defaults - its own path tracer with specular mollification,
+//   temporal accumulation, variance, 5 a-trous stages, background, albedo modulation + TAA; its output is the filtered image
+//   GFX_BUF_SVGF_FINAL of the last frame instead of the beauty buffer.
 //   -view (with a .png output): write a debug view after the last frame instead of the beauty, as the reference apps'
 //   "buffer to display" choices show it (gfx_present_launch): prediction = "Directly Visualized Prediction" (nrc: the
 //   visualizePrediction pass + inference of the primary hits, neural_radiance_caching_main.cpp:2371-2387), pathlength =
 //   "Rendering Path Length" (nrc), flow = "Motion Vector" (any renderer), cells = "Visualize Cells" (regir).
-// Output: the accumulated beauty buffer (float4 per pixel, row-major) after <frames> frames, plus one line of JSON
+// Output: the accumulated beauty buffer (svgf: the filtered image) (float4 per pixel, row-major) after <frames> frames, plus one line of JSON
 // with the mean milliseconds per frame (wall clock around a synchronised loop).
 #include "gfxb200.h"
 #include "png_writer.h"
@@ -257,6 +260,23 @@ int main(int argc, char** argv) {
                 check(gfx, gfx_nrc_shuffle(gfx, nullptr, &fp), "shuffleTrainingData");
                 check(gfx, gfx_nrc_frame_train(gfx, nrc, nullptr, nullptr), "neuralRadianceCache.train");
             }
+            else if (renderer == "svgf") {                                                 // svgf_main.cpp:1980-2172
+                constexpr uint32_t numFilteringStages = 5;
+                fp.svgfFlags |= GFX_SVGF_ENABLE_TEMPORAL_ACCUMULATION | GFX_SVGF_MOLLIFY_SPECULAR;  // the app's defaults (:1729-1733)
+                if (newSequence)
+                    fp.svgfFlags |= GFX_SVGF_IS_FIRST_FRAME;
+                else
+                    fp.svgfFlags &= ~(uint32_t)GFX_SVGF_IS_FIRST_FRAME;
+                check(gfx, gfx_gbuffer_launch(gfx, nullptr, &fp), "gfx_gbuffer_launch");
+                check(gfx, gfx_pathtrace_launch(gfx, nullptr, &fp, GFX_PT_SVGF), "pathTraceWithTemporalAccumulation");
+                check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_TEMPORAL_ACCUMULATE, 0), "temporal accumulation");
+                check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_ESTIMATE_VARIANCE, 0), "estimateVariance");
+                for (uint32_t stage = 0; stage < numFilteringStages; ++stage)
+                    check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_ATROUS, stage), "applyATrousFilter_box3x3");
+                check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_FILL_BACKGROUND, numFilteringStages), "fillBackground");
+                check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_MODULATE_TAA, numFilteringStages),
+                      "applyAlbedoModulationAndTemporalAntiAliasing");
+            }
             else {
                 throw std::runtime_error("unknown renderer " + renderer);
             }
@@ -264,10 +284,13 @@ int main(int argc, char** argv) {
             totalMs += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         }
 
+        // the svgf renderer shows the filtered image of the last frame's temporal set
+        const int outBuffer = renderer == "svgf" ? GFX_BUF_SVGF_FINAL : GFX_BUF_BEAUTY_ACCUM;
+        const uint32_t outIndex = renderer == "svgf" ? fp.bufferIndex : 0u;
         if (pngOut) {
             // the reference's screenshot: tone map + sRGB gamma on the accumulated beauty (saveImage with
             // SDRImageSaverConfig, common_host.cpp:2859-2897; brightness 0 -> scale 10^0), written as PNG
-            GfxPresentParams pp = { GFX_BUF_BEAUTY_ACCUM, 0, GFX_PRESENT_COLOR, GFX_PRESENT_TONE_MAP | GFX_PRESENT_SRGB_GAMMA, 1.0f, 1.0f,
+            GfxPresentParams pp = { outBuffer, outIndex, GFX_PRESENT_COLOR, GFX_PRESENT_TONE_MAP | GFX_PRESENT_SRGB_GAMMA, 1.0f, 1.0f,
                                     &fp, 0.1f, 0.5f };  // motion vectors x 10^-1 + 0.5 (neural_radiance_caching_main.cpp:2462)
             if (view == "prediction") {                                                    // :2371-2387
                 check(gfx, gfx_pathtrace_launch(gfx, nullptr, &fp, GFX_PT_NRC_VISUALIZE_PREDICTION), "visualizePrediction");
@@ -288,7 +311,7 @@ int main(int argc, char** argv) {
         }
         else {
             std::vector<float> beauty((size_t)width * height * 4);
-            check(gfx, gfx_buffer_download(gfx, nullptr, GFX_BUF_BEAUTY_ACCUM, 0, beauty.data(), beauty.size() * 4), "gfx_buffer_download");
+            check(gfx, gfx_buffer_download(gfx, nullptr, outBuffer, outIndex, beauty.data(), beauty.size() * 4), "gfx_buffer_download");
             FILE* of = fopen(outPath.c_str(), "wb");
             if (!of || fwrite(beauty.data(), 4, beauty.size(), of) != beauty.size())
                 throw std::runtime_error("cannot write the output image");

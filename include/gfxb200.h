@@ -245,7 +245,9 @@ typedef enum GfxSVGFFlags {
     GFX_SVGF_ENABLE_TEMPORAL_ACCUMULATION = 2,
     GFX_SVGF_FEEDBACK_1ST_FILTERED_RESULT = 4,
     GFX_SVGF_ENABLE_TEMPORAL_AA = 8,
-    GFX_SVGF_MODULATE_ALBEDO = 16
+    GFX_SVGF_MODULATE_ALBEDO = 16,
+    GFX_SVGF_MOLLIFY_SPECULAR = 32    /* mollifySpecular (svgf_shared.h:225, svgf_main.cpp:1733, 1995; on in the SVGF app by default):
+                                       * GFX_PT_SVGF sets up the BSDFs of the bounces (not of the first vertex) regularised */
 } GfxSVGFFlags;
 
 /* ReSTIR DI entry points (restir_di/restir_di_main.cpp:63-74 ReSTIREntryPoint) */
@@ -272,7 +274,7 @@ typedef enum GfxPathTraceVariant {
                                                  * needs gfx_nrc_preprocess first; fills the NRC buffers below */
     GFX_PT_REGIR = 2,                           /* regir's pathTraceReGIR (regir_main.cpp:2051-2057): NEE resamples the
                                                  * cell reservoirs built by gfx_regir_build_cells */
-    GFX_PT_NRC_VISUALIZE_PREDICTION = 3         /* visualizePrediction (neural_radiance_caching/gpu_kernels/
+    GFX_PT_NRC_VISUALIZE_PREDICTION = 3,        /* visualizePrediction (neural_radiance_caching/gpu_kernels/
                                                  * optix_pathtracing_kernels.cu:702-778): for every pixel of the G-buffer
                                                  * params->bufferIndex (the whole frame), a primary hit writes its radiance
                                                  * query to row y * W + x of GFX_BUF_NRC_INFERENCE_QUERY (a miss leaves its row
@@ -284,6 +286,15 @@ typedef enum GfxPathTraceVariant {
                                                  * buffers (gfx_nrc_preprocess creates them), GFX_ERR_UNSUPPORTED on a context
                                                  * sharded with gfx_nrc_shard(world > 1).  The next NRC frame overwrites
                                                  * everything it writes. */
+    GFX_PT_SVGF = 4                             /* the SVGF app's path tracer (svgf/gpu_kernels/optix_pathtracing_kernels.cu:
+                                                 * 130-513, svgf_main.cpp:2118-2126) up to its temporal accumulation, which is
+                                                 * GFX_SVGF_TEMPORAL_ACCUMULATE: from the G-buffer params->bufferIndex it writes
+                                                 * one sample of max(contribution, 0) per pixel to GFX_BUF_BEAUTY_ACCUM and the
+                                                 * first vertex's DH-reflectance estimate to GFX_BUF_ALBEDO_ACCUM (0 for a miss;
+                                                 * params->numAccumFrames is not used).  The first vertex takes the G-buffer's
+                                                 * shading normal as its geometric normal and frame; no Russian roulette at path
+                                                 * length 2; GFX_SVGF_MOLLIFY_SPECULAR in params->svgfFlags regularises the
+                                                 * bounces' BSDFs.  Rows params->tileOriginY / tileRows. */
 } GfxPathTraceVariant;
 
 /* SVGF entry points (svgf/svgf_main.cpp:2127-2172) */
@@ -292,7 +303,10 @@ typedef enum GfxSVGFPass {
     GFX_SVGF_ESTIMATE_VARIANCE = 1,   /* estimateVariance (svgf.cu:30-134) */
     GFX_SVGF_ATROUS = 2,              /* applyATrousFilter_box3x3(stage) (svgf.cu:221-354) */
     GFX_SVGF_FILL_BACKGROUND = 3,     /* fillBackground (svgf.cu:378-461) */
-    GFX_SVGF_MODULATE_TAA = 4         /* applyAlbedoModulationAndTemporalAntiAliasing (svgf.cu:533-611) */
+    GFX_SVGF_MODULATE_TAA = 4,        /* applyAlbedoModulationAndTemporalAntiAliasing (svgf.cu:533-611) */
+    GFX_SVGF_FEEDBACK_NOISY_LIGHTING = 5 /* feedbackNoisyLighting (svgf.cu:356-374): lighting plane 0 -> GFX_BUF_SVGF_PREV_LIGHTING,
+                                          * the SVGF app's frame with SVGF off and temporal accumulation on (svgf_main.cpp:2159-2164);
+                                          * FILL_BACKGROUND / MODULATE_TAA then take stage 0 */
 } GfxSVGFPass;
 
 /* buffers that can be read back for parity checks (logical row-major (x,y) order) */
