@@ -110,7 +110,7 @@ NRC_POSITION_ENCODING_TRIANGLE_WAVE, NRC_POSITION_ENCODING_HASH_GRID = 0, 1  # g
 (SVGF_TEMPORAL_ACCUMULATE, SVGF_ESTIMATE_VARIANCE, SVGF_ATROUS, SVGF_FILL_BACKGROUND, SVGF_MODULATE_TAA,
  SVGF_FEEDBACK_NOISY_LIGHTING) = range(6)
 (SVGF_IS_FIRST_FRAME, SVGF_ENABLE_TEMPORAL_ACCUMULATION, SVGF_FEEDBACK_1ST, SVGF_ENABLE_TAA, SVGF_MODULATE_ALBEDO,
- SVGF_MOLLIFY_SPECULAR) = 1, 2, 4, 8, 16, 32
+ SVGF_MOLLIFY_SPECULAR, SVGF_SUBPIXEL_JITTER) = 1, 2, 4, 8, 16, 32, 64
 (BUF_GBUFFER0, BUF_GBUFFER1, BUF_GBUFFER2, BUF_GBUFFER3, BUF_RNG, BUF_RESERVOIR, BUF_RESERVOIR_INFO,
  BUF_BEAUTY_ACCUM, BUF_ALBEDO_ACCUM, BUF_NORMAL_ACCUM, BUF_SVGF_LIGHTING_VARIANCE, BUF_SVGF_FINAL,
  BUF_SVGF_MOMENTS, BUF_SVGF_PREV_LIGHTING, BUF_SVGF_ALBEDO, BUF_SVGF_DEPTH,

@@ -121,6 +121,31 @@ DevFrameParams makeDevParams(const gfx_ctx* ctx, const GfxFrameParams* p) {
     return d;
 }
 
+int svgfSubPixelSample(gfx_ctx* ctx, const GfxFrameParams* p, bool* jitter, float2* sample) {
+    *jitter = false;
+    *sample = make_float2(0.5f, 0.5f);
+    if (!(p->svgfFlags & GFX_SVGF_SUBPIXEL_JITTER))
+        return GFX_OK;
+    if (p->enableJittering) {
+        ctx->setError("GFX_SVGF_SUBPIXEL_JITTER and enableJittering both move the primary ray's sample: set one of them");
+        return GFX_ERR_INVALID_ARGUMENT;
+    }
+    if (!(p->svgfFlags & GFX_SVGF_ENABLE_TEMPORAL_AA)) // svgf_main.cpp:2005-2007: the pixel centre without TAA
+        return GFX_OK;
+    // subPixelOffsets[frameIndex % taaHistoryLength] (svgf_main.cpp:1422-1424, 2007)
+    const uint32_t taaHistoryLength = p->taaHistoryLength ? p->taaHistoryLength : 16;
+    const uint32_t i = p->frameIndex % taaHistoryLength;
+    const float ox = dm_halton(2, i), oy = dm_halton(3, i);
+    // The app rasterises the G-buffer with addOffset(matV2C, ox, oy) (svgf_main.cpp:2015-2028): clip x gains
+    // (2 ox - 1) / W times view z, so after the divide by w = -z the fragment at GL pixel centre X + 0.5 shows the point whose
+    // unjittered projection lies at X + ox; likewise Y + oy in y.  The qRotateY(pi) of matW2V makes GL's x run the way this
+    // library's x does, and GL counts rows from the bottom: GL row Y is row y = H - 1 - Y here, so the sample lies at
+    // H - (Y + oy) = y + 1 - oy.  fillBackground (svgf.cu:406-408) writes the same position.
+    *jitter = true;
+    *sample = make_float2(ox, 1.0f - oy);
+    return GFX_OK;
+}
+
 } // namespace gfx
 
 DevScene gfx_ctx::devScene() const {

@@ -295,4 +295,8 @@ int launchNrcPreprocess(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams*
                         uint32_t offsetToSelectTrainingPath, int isNewSequence);
 int launchNrcPass(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int pass); // 0 accumulate, 1 propagate, 2 shuffle
 DevFrameParams makeDevParams(const gfx_ctx* ctx, const GfxFrameParams* p);
+// GFX_SVGF_SUBPIXEL_JITTER: *jitter tells whether it applies to the frame (only with GFX_SVGF_ENABLE_TEMPORAL_AA), and then
+// *sample = (ox, 1 - oy) is the sample's offset from the pixel's top-left corner in top-down pixel coordinates.  Refuses a
+// frame that also sets enableJittering (GFX_ERR_INVALID_ARGUMENT).
+int svgfSubPixelSample(gfx_ctx* ctx, const GfxFrameParams* p, bool* jitter, float2* sample);
 } // namespace gfx

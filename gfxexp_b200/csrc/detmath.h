@@ -54,6 +54,20 @@ DM_HD int32_t dm_f2int(float f) {
     return (int32_t)f;
 }
 
+// Radical inverse of idx in base `base`, the float loop of svgf_main.cpp:1410-1421 that fills the SVGF app's table of TAA
+// sub-pixel offsets.  The reference's build rounds every step (MSVC /fp:precise); so must every compiler here.
+DM_HD float dm_halton(uint32_t base, uint32_t idx) {
+    const float recBase = 1.0f / base;
+    float ret = 0.0f;
+    float scale = 1.0f;
+    while (idx) {
+        scale *= recBase;
+        ret += (idx % base) * scale;
+        idx /= base;
+    }
+    return ret;
+}
+
 // sin and cos of x (|x| up to a few thousand; the path only feeds [-pi, 4pi]).
 // Quadrant reduction by pi/2 with a three-term Cody-Waite split, then the Cephes minimax
 // polynomials on [-pi/4, pi/4].

@@ -31,7 +31,9 @@ GFX_D void countRays(const DevFrame &frame, uint32_t n) {
         atomicAdd(frame.stats, (unsigned long long)total);
 }
 
-GFX_D uint32_t gbufferPixel(const DevScene &scene, const DevFrame &frame, const DevFrameParams &p) {
+// JITTER: GFX_SVGF_SUBPIXEL_JITTER, the primary ray through (x, y) + sample (svgfSubPixelSample) and no random number drawn
+template <bool JITTER>
+GFX_D uint32_t gbufferPixel(const DevScene &scene, const DevFrame &frame, const DevFrameParams &p, float2 sample) {
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
     const uint32_t y = p.y0 + blockIdx.y * 8 + threadIdx.y;
     if (x >= frame.W || y >= p.y1)
@@ -40,7 +42,11 @@ GFX_D uint32_t gbufferPixel(const DevScene &scene, const DevFrame &frame, const 
     const uint32_t bufIdx = p.bufferIndex;
 
     float jx = 0.5f, jy = 0.5f;
-    if (p.enableJittering) {
+    if (JITTER) {
+        jx = sample.x;
+        jy = sample.y;
+    }
+    else if (p.enableJittering) {
         PCG32RNG rng{ frame.rng[pix] };
         jx = rng.getFloat0cTo1o();
         jy = rng.getFloat0cTo1o();
@@ -135,8 +141,10 @@ GFX_D uint32_t gbufferPixel(const DevScene &scene, const DevFrame &frame, const 
         qbcC = encodeBarycentric(v);
     }
 
-    // ray-gen epilogue (:56-109)
-    const f2 curRasterPos(x + 0.5f, y + 0.5f);
+    // ray-gen epilogue (:56-109).  With the jitter the current raster position is the sample's: it is where the point
+    // projects without the offset, and GL's prevScreenPos = pixel centre - (that - previous projection) is what
+    // k_svgfTemporal computes from this motion vector.
+    const f2 curRasterPos = JITTER ? f2(x + jx, y + jy) : f2(x + 0.5f, y + 0.5f);
     const f2 prevRasterPos = calcScreenPosition(p.prevCamera, prevPositionInWorld) * f2((float)frame.W, (float)frame.H);
     f2 motionVector = curRasterPos - prevRasterPos;
     if (p.resetFlowBuffer || isnan(prevPositionInWorld.x))
@@ -162,17 +170,29 @@ GFX_D uint32_t gbufferPixel(const DevScene &scene, const DevFrame &frame, const 
 }
 
 __global__ void __launch_bounds__(64) k_gbuffer(DevScene scene, DevFrame frame, DevFrameParams p) {
-    countRays(frame, gbufferPixel(scene, frame, p));
+    countRays(frame, gbufferPixel<false>(scene, frame, p, make_float2(0.5f, 0.5f)));
+}
+
+__global__ void __launch_bounds__(64) k_gbufferSubPixelJitter(DevScene scene, DevFrame frame, DevFrameParams p, float2 sample) {
+    countRays(frame, gbufferPixel<true>(scene, frame, p, sample));
 }
 
 int launchGBuffer(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params) {
+    bool jitter;
+    float2 sample;
+    const int rc = svgfSubPixelSample(ctx, params, &jitter, &sample);
+    if (rc != GFX_OK)
+        return rc;
     const DevFrameParams p = makeDevParams(ctx, params);
     if (p.y1 <= p.y0)
         return GFX_OK;
     const dim3 block(8, 8);
     const dim3 grid((ctx->frame.W + 7) / 8, (p.y1 - p.y0 + 7) / 8);
     GFX_TIMED(ctx, stream, "gbuffer");
-    k_gbuffer<<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p);
+    if (jitter)
+        k_gbufferSubPixelJitter<<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p, sample);
+    else
+        k_gbuffer<<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p);
     ctx->launches++;
     GFX_CUDA(ctx, cudaGetLastError());
     return GFX_OK;

@@ -324,7 +324,11 @@ __global__ void __launch_bounds__(256) k_svgfATrous(DevSvgf s, DevFrameParams p,
 }
 
 // ---- fillBackground (svgf.cu:378-461) -----------------------------------------------------
-__global__ void __launch_bounds__(256) k_svgfBackground(DevSvgf s, DevFrameParams p, uint32_t numFilteringStages, DevEnvLight env) {
+// JITTER: GFX_SVGF_SUBPIXEL_JITTER, the environment seen through (x, y) + sample (computeEnvDirection(..., true), :404-408,
+// :436); prevScreenPos stays the pixel centre's (:443)
+template <bool JITTER>
+GFX_D void svgfBackgroundPixel(const DevSvgf &s, const DevFrameParams &p, uint32_t numFilteringStages, const DevEnvLight &env,
+                               float2 sample) {
     SVGF_PIXEL();
     const uint32_t curBufIdx = p.bufferIndex;
     if (s.gb0[curBufIdx][pix].x != 0xFFFFFFFFu)
@@ -333,9 +337,15 @@ __global__ void __launch_bounds__(256) k_svgfBackground(DevSvgf s, DevFrameParam
     const float fx = (x + 0.5f) / W;
     const float fy = (y + 0.5f) / H;
     f3 direction = normalize(mul3x3(p.camera.orientation, f3(p.camera.vw * (0.5f - fx), p.camera.vh * (0.5f - fy), 1)));
-    if (env.enabled) { // :431-437; the camera's sub-pixel offset is the pixel centre here (no TAA jitter in this host)
+    if (env.enabled) { // :431-437; without the jitter the camera's sub-pixel offset is the pixel centre
+        f3 envDirection = direction;
+        if (JITTER) {
+            const float jfx = (x + sample.x) / W;
+            const float jfy = (y + sample.y) / H;
+            envDirection = normalize(mul3x3(p.camera.orientation, f3(p.camera.vw * (0.5f - jfx), p.camera.vh * (0.5f - jfy), 1)));
+        }
         float posPhi, posTheta;
-        toPolarYUp(direction, &posPhi, &posTheta);
+        toPolarYUp(envDirection, &posPhi, &posTheta);
         float phi = posPhi + env.rotation;
         phi += env.rotation; // as written in the reference (:418-420): the rotation is added twice when the environment light is on
         float u = phi / (2 * kPi);
@@ -352,6 +362,15 @@ __global__ void __launch_bounds__(256) k_svgfBackground(DevSvgf s, DevFrameParam
     s.lighting[numFilteringStages % 2][pix] = make_float4(finalLighting.x, finalLighting.y, finalLighting.z, 0.0f);
     s.albedo[pix] = make_float4(1.0f, 1.0f, 1.0f, 0.0f);
     s.prevScreenPos[pix] = make_float2(prevScreenPos.x, prevScreenPos.y);
+}
+
+__global__ void __launch_bounds__(256) k_svgfBackground(DevSvgf s, DevFrameParams p, uint32_t numFilteringStages, DevEnvLight env) {
+    svgfBackgroundPixel<false>(s, p, numFilteringStages, env, make_float2(0.5f, 0.5f));
+}
+
+__global__ void __launch_bounds__(256) k_svgfBackgroundSubPixelJitter(DevSvgf s, DevFrameParams p, uint32_t numFilteringStages,
+                                                                      DevEnvLight env, float2 sample) {
+    svgfBackgroundPixel<true>(s, p, numFilteringStages, env, sample);
 }
 
 // ---- albedo modulation + TAA (svgf.cu:465-611) -------------------------------------------
@@ -448,6 +467,11 @@ __global__ void __launch_bounds__(256) k_svgfFeedbackNoisyLighting(DevSvgf s, De
 }
 
 int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int pass, uint32_t stage) {
+    bool jitter;
+    float2 sample;
+    const int rc = svgfSubPixelSample(ctx, params, &jitter, &sample);
+    if (rc != GFX_OK)
+        return rc;
     const DevFrameParams p = makeDevParams(ctx, params);
     if (p.y1 <= p.y0)
         return GFX_OK;
@@ -491,7 +515,13 @@ int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, 
         }
         { GFX_TIMED(ctx, stream, "svgf_atrous"); k_svgfATrous<<<grid, block, 0, stream>>>(s, p, stage); }
         break;
-    case GFX_SVGF_FILL_BACKGROUND: { GFX_TIMED(ctx, stream, "svgf_background"); k_svgfBackground<<<grid, block, 0, stream>>>(s, p, stage, ctx->devScene(params).env); } break;
+    case GFX_SVGF_FILL_BACKGROUND: {
+        GFX_TIMED(ctx, stream, "svgf_background");
+        if (jitter)
+            k_svgfBackgroundSubPixelJitter<<<grid, block, 0, stream>>>(s, p, stage, ctx->devScene(params).env, sample);
+        else
+            k_svgfBackground<<<grid, block, 0, stream>>>(s, p, stage, ctx->devScene(params).env);
+    } break;
     case GFX_SVGF_MODULATE_TAA: { GFX_TIMED(ctx, stream, "svgf_modulate_taa"); k_svgfModulateTAA<<<grid, block, 0, stream>>>(s, p, stage); } break;
     case GFX_SVGF_FEEDBACK_NOISY_LIGHTING: { GFX_TIMED(ctx, stream, "svgf_feedback_noisy_lighting"); k_svgfFeedbackNoisyLighting<<<grid, block, 0, stream>>>(s, p); } break;
     default:

@@ -467,7 +467,7 @@ def svgf_frame_passes(params, frame_index: int, num_filtering_stages: int = 5):
 
 
 def svgf_app_frame_passes(params, frame_index: int, enable_svgf: bool = True, temporal_accumulation: bool = True,
-                          mollify: bool = True, num_filtering_stages: int = 5):
+                          mollify: bool = True, num_filtering_stages: int = 5, taa_jitter: bool = False):
     """The launch list of one frame of the SVGF app (svgf/svgf_main.cpp:1980-2172): light distributions, G-buffer, the app's
     own path tracer (GFX_PT_SVGF), temporal accumulation, then variance + num_filtering_stages a-trous stages with SVGF on,
     or feedbackNoisyLighting with SVGF off and temporal accumulation on, and last background fill + albedo modulation / TAA,
@@ -475,17 +475,21 @@ def svgf_app_frame_passes(params, frame_index: int, enable_svgf: bool = True, te
     "light_dist" (pass_id = buffer index), "gbuffer", "pathtrace" (pass_id = abi.PT_SVGF) or "svgf"; sets frameIndex,
     bufferIndex, the svgfFlags of the app's switches (isFirstFrame, enableTemporalAccumulation, mollifySpecular) and
     resetFlowBuffer (the G-buffer's motion vectors, which the reprojections read, are zero on a new sequence only) in `params`
-    as the host does."""
+    as the host does.  taa_jitter sets GFX_SVGF_SUBPIXEL_JITTER, the app's TAA sub-pixel jitter (svgf_main.cpp:2005-2008),
+    which applies while params.svgfFlags has GFX_SVGF_ENABLE_TEMPORAL_AA; off by default."""
     params.frameIndex = frame_index
     params.bufferIndex = frame_index % 2
     params.resetFlowBuffer = 1 if frame_index == 0 else 0
-    flags = params.svgfFlags & ~(abi.SVGF_IS_FIRST_FRAME | abi.SVGF_ENABLE_TEMPORAL_ACCUMULATION | abi.SVGF_MOLLIFY_SPECULAR)
+    flags = params.svgfFlags & ~(abi.SVGF_IS_FIRST_FRAME | abi.SVGF_ENABLE_TEMPORAL_ACCUMULATION | abi.SVGF_MOLLIFY_SPECULAR
+                                 | abi.SVGF_SUBPIXEL_JITTER)
     if frame_index == 0:
         flags |= abi.SVGF_IS_FIRST_FRAME
     if temporal_accumulation:
         flags |= abi.SVGF_ENABLE_TEMPORAL_ACCUMULATION
     if mollify:
         flags |= abi.SVGF_MOLLIFY_SPECULAR
+    if taa_jitter:
+        flags |= abi.SVGF_SUBPIXEL_JITTER
     params.svgfFlags = flags
     yield ("light_dist", frame_index % 2, 0)
     yield ("gbuffer", -1, 0)

@@ -8,7 +8,7 @@
 // types.  Scene and default parameters come from a flat binary file written by gfxexp_b200/scenes.py::save_scene_bin.
 //
 //   gfx_headless <scene.bin> <renderer> <width> <height> <frames> <out.raw> [nrc_params.f16] [-position-encoding tri|hash]
-//                [-view prediction|pathlength|flow|cells]
+//                [-view prediction|pathlength|flow|cells] [-taa-jitter]
 //   -position-encoding: the NRC network's position encoding, as the reference app's command line takes it
 //   (neural_radiance_caching_main.cpp:458, 755-766); hash grid by default.  nrc_params.f16 must hold that network's
 //   gfx_nrc_num_params halves.
@@ -16,6 +16,8 @@
 //   svgf: the SVGF app's frame (svgf_main.cpp:1980-2172) with its defaults - its own path tracer with specular mollification,
 //   temporal accumulation, variance, 5 a-trous stages, background, albedo modulation + TAA; its output is the filtered image
 //   GFX_BUF_SVGF_FINAL of the last frame instead of the beauty buffer.
+//   -taa-jitter (svgf): the app's TAA sub-pixel jitter, GFX_SVGF_SUBPIXEL_JITTER; the app sets it whenever enableTemporalAA is on
+//   (svgf_main.cpp:2005-2008), the library computes the offsets.
 //   -view (with a .png output): write a debug view after the last frame instead of the beauty, as the reference apps'
 //   "buffer to display" choices show it (gfx_present_launch): prediction = "Directly Visualized Prediction" (nrc: the
 //   visualizePrediction pass + inference of the primary hits, neural_radiance_caching_main.cpp:2371-2387), pathlength =
@@ -108,12 +110,13 @@ void loadScene(const char* path, uint32_t width, uint32_t height, SceneFile* s) 
 int main(int argc, char** argv) {
     if (argc < 7) {
         fprintf(stderr, "usage: %s <scene.bin> <renderer> <width> <height> <frames> <out.raw | out.png> [nrc_params.f16] "
-                "[-position-encoding tri|hash] [-view prediction|pathlength|flow|cells]\n", argv[0]);
+                "[-position-encoding tri|hash] [-view prediction|pathlength|flow|cells] [-taa-jitter]\n", argv[0]);
         return 2;
     }
     const char* nrcParamsPath = nullptr;
     int positionEncoding = GFX_NRC_POSITION_ENCODING_HASH_GRID;
     std::string view;
+    bool taaJitter = false;
     for (int i = 7; i < argc; ++i) {
         const std::string arg = argv[i];
         if (arg == "-position-encoding" && i + 1 < argc) {
@@ -134,6 +137,8 @@ int main(int argc, char** argv) {
                 return 2;
             }
         }
+        else if (arg == "-taa-jitter")
+            taaJitter = true;
         else if (!nrcParamsPath && arg[0] != '-')
             nrcParamsPath = argv[i];
         else {
@@ -148,6 +153,10 @@ int main(int argc, char** argv) {
                           (view == "cells" && renderer != "regir"))) {
         fprintf(stderr, "-view %s needs a .png output and %s\n", view.c_str(),
                 view == "cells" ? "the regir renderer" : view == "flow" ? "nothing else" : "the nrc renderer");
+        return 2;
+    }
+    if (taaJitter && renderer != "svgf") {
+        fprintf(stderr, "-taa-jitter needs the svgf renderer\n");
         return 2;
     }
     const uint32_t width = (uint32_t)atoi(argv[3]), height = (uint32_t)atoi(argv[4]);
@@ -263,6 +272,8 @@ int main(int argc, char** argv) {
             else if (renderer == "svgf") {                                                 // svgf_main.cpp:1980-2172
                 constexpr uint32_t numFilteringStages = 5;
                 fp.svgfFlags |= GFX_SVGF_ENABLE_TEMPORAL_ACCUMULATION | GFX_SVGF_MOLLIFY_SPECULAR;  // the app's defaults (:1729-1733)
+                if (taaJitter)
+                    fp.svgfFlags |= GFX_SVGF_SUBPIXEL_JITTER;  // :2005-2008, with enableTemporalAA (on in the scene file's defaults)
                 if (newSequence)
                     fp.svgfFlags |= GFX_SVGF_IS_FIRST_FRAME;
                 else

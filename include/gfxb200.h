@@ -246,8 +246,16 @@ typedef enum GfxSVGFFlags {
     GFX_SVGF_FEEDBACK_1ST_FILTERED_RESULT = 4,
     GFX_SVGF_ENABLE_TEMPORAL_AA = 8,
     GFX_SVGF_MODULATE_ALBEDO = 16,
-    GFX_SVGF_MOLLIFY_SPECULAR = 32    /* mollifySpecular (svgf_shared.h:225, svgf_main.cpp:1733, 1995; on in the SVGF app by default):
+    GFX_SVGF_MOLLIFY_SPECULAR = 32,   /* mollifySpecular (svgf_shared.h:225, svgf_main.cpp:1733, 1995; on in the SVGF app by default):
                                        * GFX_PT_SVGF sets up the BSDFs of the bounces (not of the first vertex) regularised */
+    GFX_SVGF_SUBPIXEL_JITTER = 64     /* the SVGF app's TAA sub-pixel jitter (svgf_main.cpp:1410-1424, 2005-2008); only together
+                                       * with GFX_SVGF_ENABLE_TEMPORAL_AA, as in the app.  The library computes the offset
+                                       * (ox, oy) = (halton(2, i), halton(3, i)), i = frameIndex % taaHistoryLength (0 means 16);
+                                       * the app's table has 256 entries, so a taaHistoryLength above 256 goes beyond what the app
+                                       * can run.  gfx_gbuffer_launch casts the primary ray through (x + ox, y + 1 - oy) in
+                                       * top-down pixel coordinates and measures the motion vector from that sample position, and
+                                       * GFX_SVGF_FILL_BACKGROUND looks the environment up through it; no random number is drawn.
+                                       * A frame that also sets enableJittering is refused with GFX_ERR_INVALID_ARGUMENT. */
 } GfxSVGFFlags;
 
 /* ReSTIR DI entry points (restir_di/restir_di_main.cpp:63-74 ReSTIREntryPoint) */

@@ -4,8 +4,10 @@ app's path tracer (GFX_PT_SVGF, maxPathLength 5, specular mollification on), tem
 stages, background, albedo modulation + TAA.  After warm-up, CUDA events time whole frames; gfx_timing_enable /
 gfx_timing_read give the per-kernel times of one more pass over as many frames, and the device ray counter, read around
 every path tracer launch of that pass, its rays.  Prints one JSON line with the card's name and power limit, read in the same call.
+--taa-jitter turns on the app's TAA sub-pixel jitter (GFX_SVGF_SUBPIXEL_JITTER), which moves the G-buffer's primary rays and
+the background's environment lookups off the pixel centres.
 
-    python tools/svgf_app_bench.py [--frames N] [--warmup W] [--small]
+    python tools/svgf_app_bench.py [--frames N] [--warmup W] [--small] [--taa-jitter]
 """
 import argparse
 import json
@@ -33,6 +35,7 @@ def main():
     ap.add_argument("--frames", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--small", action="store_true", help="small city at 640x360 (a quick check, not the reported figure)")
+    ap.add_argument("--taa-jitter", action="store_true", help="the app's TAA sub-pixel jitter (GFX_SVGF_SUBPIXEL_JITTER)")
     args = ap.parse_args()
     scene = scenes.small_city_scene() if args.small else scenes.bistro_class_scene()
     w, h = (640, 360) if args.small else (1920, 1080)
@@ -49,7 +52,7 @@ def main():
     def run(n, count_rays=False):
         nonlocal frame
         for _ in range(n):
-            for kind, pass_id, stage in engine.svgf_app_frame_passes(p, frame, mollify=True):
+            for kind, pass_id, stage in engine.svgf_app_frame_passes(p, frame, mollify=True, taa_jitter=args.taa_jitter):
                 if count_rays and kind == "pathtrace":
                     ctx.read_stats(reset=True)  # the G-buffer's primary rays go to the same counter
                 engine.run_svgf_app_pass(ctx, p, kind, pass_id, stage)
@@ -76,7 +79,7 @@ def main():
     ctx.timing_enable(False)
     pt_ms = sum(v for k, v in kernels.items() if k.startswith("pt_"))
     print(json.dumps({"bench": "svgf_app_frame", "scene": scene.name, "width": w, "height": h, "max_path_length": 5,
-                      "mollify_specular": True, "frames": args.frames, "warmup": args.warmup, "frame_ms": round(frame_ms, 4),
+                      "mollify_specular": True, "taa_jitter": args.taa_jitter, "frames": args.frames, "warmup": args.warmup, "frame_ms": round(frame_ms, 4),
                       "pathtrace_ms": round(pt_ms, 4), "pathtrace_rays_per_frame": rays,
                       "pathtrace_Mrays_per_s": round(rays / (pt_ms * 1e-3) / 1e6, 1) if pt_ms > 0 else None,
                       "kernel_ms": kernels, "gpu": torch.cuda.get_device_name(0), "power_limit_w": _power_limit_w()}))
