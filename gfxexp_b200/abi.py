@@ -121,6 +121,10 @@ NRC_POSITION_ENCODING_TRIANGLE_WAVE, NRC_POSITION_ENCODING_HASH_GRID = 0, 1  # g
 
 # logical per-pixel layout of each downloadable buffer: (numpy dtype, elements per pixel, planes)
 BUF_PRESENT_RGBA8 = 33
+BUF_SVGF_DEBUG_VISUALIZE = 34  # gfx_svgf_debug_visualize output
+# GfxSVGFView, the SVGF app's shared::BufferToDisplay without FinalRendering (the present of BUF_SVGF_FINAL)
+(SVGF_VIEW_NOISY_BEAUTY, SVGF_VIEW_VARIANCE, SVGF_VIEW_FILTERED_VARIANCE, SVGF_VIEW_ALBEDO, SVGF_VIEW_NORMAL,
+ SVGF_VIEW_MOTION_VECTOR, SVGF_VIEW_SAMPLE_COUNT) = range(7)
 PRESENT_COLOR, PRESENT_NORMAL, PRESENT_NRC_PREDICTION, PRESENT_NRC_PATH_LENGTH, PRESENT_FLOW = 0, 1, 2, 3, 4
 PRESENT_TONE_MAP, PRESENT_SRGB_GAMMA, PRESENT_FLIP_Y, PRESENT_NRC_TRAINING_PATHS, PRESENT_REGIR_CELLS = 1, 2, 4, 8, 16
 BUF_PEER_FLAGS = -1  # GFX_BUF_PEER_FLAGS: the flag block of the peer exchange (csrc/peer.cu)
@@ -133,6 +137,7 @@ BUFFER_LAYOUT = {
     BUF_SVGF_LIGHTING_VARIANCE: (np.float32, 4, 1), BUF_SVGF_FINAL: (np.float32, 4, 1),
     BUF_SVGF_MOMENTS: (np.uint32, 4, 1), BUF_SVGF_PREV_LIGHTING: (np.float32, 4, 1),
     BUF_SVGF_ALBEDO: (np.float32, 4, 1), BUF_SVGF_DEPTH: (np.float32, 1, 1), BUF_PRESENT_RGBA8: (np.uint32, 1, 1),
+    BUF_SVGF_DEBUG_VISUALIZE: (np.float32, 4, 1),
 }
 
 
@@ -389,6 +394,7 @@ _DECLS = {
     "gfx_gbuffer_launch": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GfxFrameParams)]),
     "gfx_restir_launch": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GfxFrameParams), C.c_int]),
     "gfx_svgf_launch": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GfxFrameParams), C.c_int, c_u32]),
+    "gfx_svgf_debug_visualize": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GfxFrameParams), C.c_int, c_f, c_f, c_u32]),
     "gfx_pathtrace_launch": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GfxFrameParams), C.c_int]),
     "gfx_timing_enable": (C.c_int, [C.c_void_p, C.c_int]),
     "gfx_timing_read": (C.c_int, [C.c_void_p, C.c_void_p, c_u32, C.POINTER(c_u32)]),

@@ -47,7 +47,7 @@ void FrameState::release() {
     cudaFree(rayQueue); cudaFree(rayPixel); cudaFree(rayCounters); cudaFree(visibility);
     cudaFree(presentRgba8);
     cudaFree(stats); cudaFree(rng); cudaFree(beauty); cudaFree(albedo); cudaFree(normal); cudaFree(neighborDeltas);
-    cudaFree(svgfPrevLighting); cudaFree(svgfAlbedo); cudaFree(svgfPrevScreenPos); cudaFree(svgfNormal);
+    cudaFree(svgfPrevLighting); cudaFree(svgfAlbedo); cudaFree(svgfPrevScreenPos); cudaFree(svgfNormal); cudaFree(svgfDebugVisualize);
     cudaFree(ptAlphaPdf); cudaFree(ptRadiance); cudaFree(ptExtHits); cudaFree(ptShadowPending); cudaFree(ptCounters);
     cudaFree(rearch.preSampledLights); cudaFree(rearch.rngs); cudaFree(rearch.sampleVis[0]); cudaFree(rearch.sampleVis[1]);
     cudaFree(rearch.rays); cudaFree(rearch.rayPixel); cudaFree(rearch.rayMask); cudaFree(rearch.counters);
@@ -900,6 +900,7 @@ static void* bufferPtr(gfx_ctx* ctx, int id, uint32_t index, size_t* bytes) {
     case GFX_BUF_SVGF_PREV_LIGHTING: p = F.svgfPrevLighting; b = n * 16; break;
     case GFX_BUF_SVGF_ALBEDO: p = F.svgfAlbedo; b = n * 16; break;
     case GFX_BUF_SVGF_DEPTH: p = F.svgfDepth[i]; b = n * 4; break;
+    case GFX_BUF_SVGF_DEBUG_VISUALIZE: p = F.svgfDebugVisualize; b = F.svgfDebugVisualize ? n * 16 : 0; break;
     default: break;
     }
     if (id >= GFX_BUF_NRC_INFERENCE_QUERY && id <= GFX_BUF_NRC_STATE) {
@@ -1024,6 +1025,17 @@ int gfx_svgf_launch(gfx_ctx* ctx, void* stream, const GfxFrameParams* params, in
     if (!ctx->frame.created)
         return GFX_ERR_NOT_READY;
     return launchSVGF(ctx, (cudaStream_t)stream, params, pass, stage);
+}
+
+int gfx_svgf_debug_visualize(gfx_ctx* ctx, void* stream, const GfxFrameParams* params, int view, float motionVectorOffset,
+                             float motionVectorScale, uint32_t numFilteringStages) {
+    CHECK_CTX(ctx);
+    if (!params)
+        return GFX_ERR_INVALID_ARGUMENT;
+    if (!ctx->frame.created)
+        return GFX_ERR_NOT_READY;
+    return launchSVGFDebugVisualize(ctx, (cudaStream_t)stream, params, view, motionVectorOffset, motionVectorScale,
+                                    numFilteringStages);
 }
 
 int gfx_pathtrace_launch(gfx_ctx* ctx, void* stream, const GfxFrameParams* params, int variant) {

@@ -186,6 +186,7 @@ struct FrameState {
     float2* svgfPrevScreenPos = nullptr;
     float4* svgfFinal[2] = { nullptr, nullptr };
     float* svgfDepth[2] = { nullptr, nullptr };
+    float4* svgfDebugVisualize = nullptr; // gfx_svgf_debug_visualize output, allocated on first use
     bool created = false;
     void release();
 };
@@ -281,6 +282,8 @@ int launchReSTIR(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int
 int launchReSTIRRearch(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int pass);
 int ensureRearch(gfx_ctx* ctx, uint32_t raysPerPixel);
 int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int pass, uint32_t stage);
+int launchSVGFDebugVisualize(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int view, float motionVectorOffset,
+                             float motionVectorScale, uint32_t numFilteringStages);
 int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int variant);
 int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p);
 int launchNrcVisualizePrediction(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p);

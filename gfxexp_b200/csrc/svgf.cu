@@ -466,15 +466,60 @@ __global__ void __launch_bounds__(256) k_svgfFeedbackNoisyLighting(DevSvgf s, De
     s.prevLighting[pix] = s.lighting[0][pix];
 }
 
-int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int pass, uint32_t stage) {
-    bool jitter;
-    float2 sample;
-    const int rc = svgfSubPixelSample(ctx, params, &jitter, &sample);
-    if (rc != GFX_OK)
-        return rc;
-    const DevFrameParams p = makeDevParams(ctx, params);
-    if (p.y1 <= p.y0)
-        return GFX_OK;
+// ---- debugVisualize (visualize.cu:6-87) ----------------------------------------------------
+// The app reads its lighting, albedo and moment planes at the launch index and its G-buffers (normal, prevScreenPos) at
+// glPix(launch index), and writes the view at glPix(launch index).  That is the indexing of every SVGF kernel of the app:
+// applyAlbedoModulationAndTemporalAntiAliasing too reads the lighting at the launch index and writes finalLightingBuffer at
+// glPix (svgf.cu:555, 610), and the display shows both buffers through the same shader.  The planes here are top-down, like
+// GFX_BUF_SVGF_FINAL, so pixel (x, y) of every plane is pixel (x, y) of the view: no flip.
+__global__ void __launch_bounds__(256) k_svgfDebugVisualize(DevSvgf s, DevFrameParams p, float4* out, int view,
+                                                            float motionVectorOffset, float motionVectorScale,
+                                                            uint32_t numFilteringStages) {
+    SVGF_PIXEL();
+    float4 color = make_float4(0.0f, 0.0f, 0.0f, 1.0f);
+    switch (view) {
+    case GFX_SVGF_VIEW_NOISY_BEAUTY: {
+        f3 lighting = xyz(s.lighting[0][pix]);
+        if (s.svgfFlags & GFX_SVGF_MODULATE_ALBEDO)
+            lighting *= xyz(s.albedo[pix]);
+        color = make_float4(lighting.x, lighting.y, lighting.z, 1.0f);
+    } break;
+    case GFX_SVGF_VIEW_VARIANCE: {
+        const float stdDev = sqrtf(s.lighting[0][pix].w);
+        color = make_float4(stdDev, stdDev, stdDev, 1.0f);
+    } break;
+    case GFX_SVGF_VIEW_FILTERED_VARIANCE: {
+        const float stdDev = sqrtf(s.lighting[numFilteringStages % 2][pix].w);
+        color = make_float4(stdDev, stdDev, stdDev, 1.0f);
+    } break;
+    case GFX_SVGF_VIEW_ALBEDO: {
+        const float4 albedo = s.albedo[pix];
+        color = make_float4(albedo.x, albedo.y, albedo.z, 1.0f);
+    } break;
+    case GFX_SVGF_VIEW_NORMAL: {
+        const f3 n = 0.5f * xyz(s.normal[pix]) + f3(0.5f);
+        color = make_float4(n.x, n.y, n.z, 1.0f);
+    } break;
+    case GFX_SVGF_VIEW_MOTION_VECTOR: {
+        const float2 prevScreenPos = s.prevScreenPos[pix];
+        const f2 curScreenPos((x + 0.5f) / W, (y + 0.5f) / H);
+        const f2 motionVector((float)W * (curScreenPos.x - prevScreenPos.x), (float)H * (curScreenPos.y - prevScreenPos.y));
+        color = make_float4(fminf(fmaxf(motionVectorScale * motionVector.x + motionVectorOffset, 0.0f), 1.0f),
+                            fminf(fmaxf(motionVectorScale * motionVector.y + motionVectorOffset, 0.0f), 1.0f),
+                            motionVectorOffset, 1.0f);
+    } break;
+    default: { // GFX_SVGF_VIEW_SAMPLE_COUNT: the field k_svgfVariance reads
+        const uint32_t count = __float_as_uint(s.moments[p.bufferIndex][pix].z) & 0xFFFFFFu;
+        const float value = fminf(count / 255.0f, 1.0f);
+        color = make_float4(value, value, value, 1.0f);
+    } break;
+    }
+    out[pix] = color;
+}
+
+namespace {
+
+DevSvgf makeDevSvgf(const gfx_ctx* ctx, const GfxFrameParams* params) {
     const FrameState &F = ctx->frame;
     DevSvgf s;
     s.W = F.W;
@@ -502,6 +547,22 @@ int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, 
     s.m23 = -2 * farZ * nearZ / dz;
     s.svgfFlags = params->svgfFlags;
     s.taaHistoryLength = params->taaHistoryLength ? params->taaHistoryLength : 16;
+    return s;
+}
+
+} // namespace
+
+int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int pass, uint32_t stage) {
+    bool jitter;
+    float2 sample;
+    const int rc = svgfSubPixelSample(ctx, params, &jitter, &sample);
+    if (rc != GFX_OK)
+        return rc;
+    const DevFrameParams p = makeDevParams(ctx, params);
+    if (p.y1 <= p.y0)
+        return GFX_OK;
+    const FrameState &F = ctx->frame;
+    const DevSvgf s = makeDevSvgf(ctx, params);
 
     const dim3 block(32, 8);
     const dim3 grid((F.W + 31) / 32, (p.y1 - p.y0 + 7) / 8);
@@ -527,6 +588,35 @@ int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, 
     default:
         ctx->setError("gfx_svgf_launch: unknown pass");
         return GFX_ERR_INVALID_ARGUMENT;
+    }
+    ctx->launches++;
+    GFX_CUDA(ctx, cudaGetLastError());
+    return GFX_OK;
+}
+
+int launchSVGFDebugVisualize(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int view, float motionVectorOffset,
+                             float motionVectorScale, uint32_t numFilteringStages) {
+    if (view < GFX_SVGF_VIEW_NOISY_BEAUTY || view > GFX_SVGF_VIEW_SAMPLE_COUNT) {
+        ctx->setError("gfx_svgf_debug_visualize: the view must be 0..6 (GfxSVGFView); Final Rendering is the present of "
+                      "GFX_BUF_SVGF_FINAL");
+        return GFX_ERR_INVALID_ARGUMENT;
+    }
+    FrameState &F = ctx->frame;
+    if (!F.svgfDebugVisualize) {
+        const size_t n = (size_t)F.W * F.H;
+        GFX_CUDA(ctx, cudaMalloc(&F.svgfDebugVisualize, n * 16));
+        GFX_CUDA(ctx, cudaMemsetAsync(F.svgfDebugVisualize, 0, n * 16, stream));
+    }
+    const DevFrameParams p = makeDevParams(ctx, params);
+    if (p.y1 <= p.y0)
+        return GFX_OK;
+    const DevSvgf s = makeDevSvgf(ctx, params);
+    const dim3 block(32, 8);
+    const dim3 grid((F.W + 31) / 32, (p.y1 - p.y0 + 7) / 8);
+    {
+        GFX_TIMED(ctx, stream, "svgf_debug_visualize");
+        k_svgfDebugVisualize<<<grid, block, 0, stream>>>(s, p, F.svgfDebugVisualize, view, motionVectorOffset, motionVectorScale,
+                                                         numFilteringStages);
     }
     ctx->launches++;
     GFX_CUDA(ctx, cudaGetLastError());

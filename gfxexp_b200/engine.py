@@ -216,6 +216,14 @@ class Context:
     def svgf(self, params, pass_id: int, stage: int = 0, stream=None):
         self._check(self.lib.gfx_svgf_launch(self.h, stream, C.byref(params), pass_id, stage), "gfx_svgf_launch")
 
+    def svgf_debug_visualize(self, params, view: int, motion_vector_offset: float = 0.5, motion_vector_scale: float = 0.1,
+                             num_filtering_stages: int = 5, stream=None):
+        """one of the SVGF app's debug views (abi.SVGF_VIEW_*, debugVisualize) into BUF_SVGF_DEBUG_VISUALIZE on the rows of
+        params; the defaults are the app's (offset 0.5, scale 10^-1, 5 stages).  Show it with
+        present(abi.BUF_SVGF_DEBUG_VISUALIZE, flags=svgf_view_present_flags(view))"""
+        self._check(self.lib.gfx_svgf_debug_visualize(self.h, stream, C.byref(params), view, motion_vector_offset,
+                                                      motion_vector_scale, num_filtering_stages), "gfx_svgf_debug_visualize")
+
     # -- NRC frame (neural_radiance_caching_main.cpp:2270-2368) -------------------------------------
     def download_linear(self, buffer_id: int, index: int = 0, stream=None, params=None) -> np.ndarray:
         """NRC / ReGIR buffers (GFX_BUF_NRC_*, GFX_BUF_REGIR_*) as [rows, cols]"""
@@ -467,7 +475,7 @@ def svgf_frame_passes(params, frame_index: int, num_filtering_stages: int = 5):
 
 
 def svgf_app_frame_passes(params, frame_index: int, enable_svgf: bool = True, temporal_accumulation: bool = True,
-                          mollify: bool = True, num_filtering_stages: int = 5, taa_jitter: bool = False):
+                          mollify: bool = True, num_filtering_stages: int = 5, taa_jitter: bool = False, view=None):
     """The launch list of one frame of the SVGF app (svgf/svgf_main.cpp:1980-2172): light distributions, G-buffer, the app's
     own path tracer (GFX_PT_SVGF), temporal accumulation, then variance + num_filtering_stages a-trous stages with SVGF on,
     or feedbackNoisyLighting with SVGF off and temporal accumulation on, and last background fill + albedo modulation / TAA,
@@ -476,7 +484,11 @@ def svgf_app_frame_passes(params, frame_index: int, enable_svgf: bool = True, te
     bufferIndex, the svgfFlags of the app's switches (isFirstFrame, enableTemporalAccumulation, mollifySpecular) and
     resetFlowBuffer (the G-buffer's motion vectors, which the reprojections read, are zero on a new sequence only) in `params`
     as the host does.  taa_jitter sets GFX_SVGF_SUBPIXEL_JITTER, the app's TAA sub-pixel jitter (svgf_main.cpp:2005-2008),
-    which applies while params.svgfFlags has GFX_SVGF_ENABLE_TEMPORAL_AA; off by default."""
+    which applies while params.svgfFlags has GFX_SVGF_ENABLE_TEMPORAL_AA; off by default.  view (abi.SVGF_VIEW_*) adds
+    ("svgf_view", view, num_filtering_stages) where the app launches its debug view (svgf_main.cpp:2138-2145, 2175-2185): Noisy
+    Beauty and Variance after the variance estimate and only with SVGF on (with SVGF off the buffer keeps what it held), the
+    other views after albedo modulation / TAA.  The view takes num_filtering_stages with SVGF off too, as the app passes its
+    constant 5 (:2127, 2183-2184): Filtered Variance then shows plane 1 as the last frame with SVGF on left it."""
     params.frameIndex = frame_index
     params.bufferIndex = frame_index % 2
     params.resetFlowBuffer = 1 if frame_index == 0 else 0
@@ -498,12 +510,24 @@ def svgf_app_frame_passes(params, frame_index: int, enable_svgf: bool = True, te
     stages = num_filtering_stages if enable_svgf else 0
     if enable_svgf:
         yield ("svgf", abi.SVGF_ESTIMATE_VARIANCE, 0)
+        if view in (abi.SVGF_VIEW_NOISY_BEAUTY, abi.SVGF_VIEW_VARIANCE):
+            yield ("svgf_view", view, num_filtering_stages)
         for stage in range(num_filtering_stages):
             yield ("svgf", abi.SVGF_ATROUS, stage)
     elif temporal_accumulation:
         yield ("svgf", abi.SVGF_FEEDBACK_NOISY_LIGHTING, 0)
     yield ("svgf", abi.SVGF_FILL_BACKGROUND, stages)
     yield ("svgf", abi.SVGF_MODULATE_TAA, stages)
+    if view is not None and view not in (abi.SVGF_VIEW_NOISY_BEAUTY, abi.SVGF_VIEW_VARIANCE):
+        yield ("svgf_view", view, num_filtering_stages)
+
+
+def svgf_view_present_flags(view: int) -> int:
+    """the display of an SVGF debug view (svgf_main.cpp:1907-1911): tone map and sRGB gamma for Noisy Beauty, Variance and
+    Filtered Variance, the raw values for Albedo, Normal, Motion Vector and Sample Count"""
+    if view in (abi.SVGF_VIEW_NOISY_BEAUTY, abi.SVGF_VIEW_VARIANCE, abi.SVGF_VIEW_FILTERED_VARIANCE):
+        return abi.PRESENT_TONE_MAP | abi.PRESENT_SRGB_GAMMA
+    return 0
 
 
 def run_svgf_app_pass(ctx: Context, params, kind: str, pass_id: int, stage: int, stream=None):
@@ -514,6 +538,8 @@ def run_svgf_app_pass(ctx: Context, params, kind: str, pass_id: int, stage: int,
         ctx.gbuffer(params, stream)
     elif kind == "pathtrace":
         ctx.pathtrace(params, pass_id, stream)
+    elif kind == "svgf_view":
+        ctx.svgf_debug_visualize(params, pass_id, num_filtering_stages=stage, stream=stream)
     else:
         ctx.svgf(params, pass_id, stage, stream)
 

@@ -8,7 +8,8 @@
 // types.  Scene and default parameters come from a flat binary file written by gfxexp_b200/scenes.py::save_scene_bin.
 //
 //   gfx_headless <scene.bin> <renderer> <width> <height> <frames> <out.raw> [nrc_params.f16] [-position-encoding tri|hash]
-//                [-view prediction|pathlength|flow|cells] [-taa-jitter]
+//                [-view prediction|pathlength|flow|cells|noisy|variance|filtered-variance|albedo|normal|motion|samples]
+//                [-taa-jitter]
 //   -position-encoding: the NRC network's position encoding, as the reference app's command line takes it
 //   (neural_radiance_caching_main.cpp:458, 755-766); hash grid by default.  nrc_params.f16 must hold that network's
 //   gfx_nrc_num_params halves.
@@ -22,6 +23,10 @@
 //   "buffer to display" choices show it (gfx_present_launch): prediction = "Directly Visualized Prediction" (nrc: the
 //   visualizePrediction pass + inference of the primary hits, neural_radiance_caching_main.cpp:2371-2387), pathlength =
 //   "Rendering Path Length" (nrc), flow = "Motion Vector" (any renderer), cells = "Visualize Cells" (regir).
+//   The SVGF app's views (svgf only): noisy, variance, filtered-variance, albedo, normal, motion and samples = "Noisy Beauty",
+//   "Variance", "Filtered Variance", "Albedo", "Normal", "Motion Vector" and "Sample Count" (svgf_main.cpp:1823-1839): every
+//   frame launches gfx_svgf_debug_visualize where the app does (:2138-2145, 2175-2185), and the last one is presented with the
+//   app's display flags (:1907-1911).
 // Output: the accumulated beauty buffer (svgf: the filtered image) (float4 per pixel, row-major) after <frames> frames, plus one line of JSON
 // with the mean milliseconds per frame (wall clock around a synchronised loop).
 #include "gfxb200.h"
@@ -110,12 +115,14 @@ void loadScene(const char* path, uint32_t width, uint32_t height, SceneFile* s) 
 int main(int argc, char** argv) {
     if (argc < 7) {
         fprintf(stderr, "usage: %s <scene.bin> <renderer> <width> <height> <frames> <out.raw | out.png> [nrc_params.f16] "
-                "[-position-encoding tri|hash] [-view prediction|pathlength|flow|cells] [-taa-jitter]\n", argv[0]);
+                "[-position-encoding tri|hash] [-view prediction|pathlength|flow|cells|noisy|variance|filtered-variance|albedo|"
+                "normal|motion|samples] [-taa-jitter]\n", argv[0]);
         return 2;
     }
     const char* nrcParamsPath = nullptr;
     int positionEncoding = GFX_NRC_POSITION_ENCODING_HASH_GRID;
     std::string view;
+    int svgfView = -1; // GfxSVGFView of an SVGF app view
     bool taaJitter = false;
     for (int i = 7; i < argc; ++i) {
         const std::string arg = argv[i];
@@ -132,8 +139,13 @@ int main(int argc, char** argv) {
         }
         else if (arg == "-view" && i + 1 < argc) {
             view = argv[++i];
-            if (view != "prediction" && view != "pathlength" && view != "flow" && view != "cells") {
-                fprintf(stderr, "-view takes prediction, pathlength, flow or cells, not %s\n", view.c_str());
+            static const char* const svgfViews[] = { "noisy", "variance", "filtered-variance", "albedo", "normal", "motion", "samples" };
+            for (int v = 0; v < 7; ++v)
+                if (view == svgfViews[v])
+                    svgfView = v; // GFX_SVGF_VIEW_NOISY_BEAUTY + v
+            if (view != "prediction" && view != "pathlength" && view != "flow" && view != "cells" && svgfView < 0) {
+                fprintf(stderr, "-view takes prediction, pathlength, flow, cells, noisy, variance, filtered-variance, albedo, "
+                        "normal, motion or samples, not %s\n", view.c_str());
                 return 2;
             }
         }
@@ -150,9 +162,10 @@ int main(int argc, char** argv) {
     const std::string outPath = argv[6];
     const bool pngOut = outPath.size() > 4 && outPath.compare(outPath.size() - 4, 4, ".png") == 0;
     if (!view.empty() && (!pngOut || ((view == "prediction" || view == "pathlength") && renderer != "nrc") ||
-                          (view == "cells" && renderer != "regir"))) {
+                          (view == "cells" && renderer != "regir") || (svgfView >= 0 && renderer != "svgf"))) {
         fprintf(stderr, "-view %s needs a .png output and %s\n", view.c_str(),
-                view == "cells" ? "the regir renderer" : view == "flow" ? "nothing else" : "the nrc renderer");
+                view == "cells" ? "the regir renderer" : view == "flow" ? "nothing else" : svgfView >= 0 ? "the svgf renderer" :
+                "the nrc renderer");
         return 2;
     }
     if (taaJitter && renderer != "svgf") {
@@ -282,11 +295,15 @@ int main(int argc, char** argv) {
                 check(gfx, gfx_pathtrace_launch(gfx, nullptr, &fp, GFX_PT_SVGF), "pathTraceWithTemporalAccumulation");
                 check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_TEMPORAL_ACCUMULATE, 0), "temporal accumulation");
                 check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_ESTIMATE_VARIANCE, 0), "estimateVariance");
+                if (svgfView == GFX_SVGF_VIEW_NOISY_BEAUTY || svgfView == GFX_SVGF_VIEW_VARIANCE)  // :2138-2145
+                    check(gfx, gfx_svgf_debug_visualize(gfx, nullptr, &fp, svgfView, 0.5f, 0.1f, numFilteringStages), "debugVisualize");
                 for (uint32_t stage = 0; stage < numFilteringStages; ++stage)
                     check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_ATROUS, stage), "applyATrousFilter_box3x3");
                 check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_FILL_BACKGROUND, numFilteringStages), "fillBackground");
                 check(gfx, gfx_svgf_launch(gfx, nullptr, &fp, GFX_SVGF_MODULATE_TAA, numFilteringStages),
                       "applyAlbedoModulationAndTemporalAntiAliasing");
+                if (svgfView > GFX_SVGF_VIEW_VARIANCE)  // :2175-2185; offset 0.5, scale 10^-1 (:1724, 2143)
+                    check(gfx, gfx_svgf_debug_visualize(gfx, nullptr, &fp, svgfView, 0.5f, 0.1f, numFilteringStages), "debugVisualize");
             }
             else {
                 throw std::runtime_error("unknown renderer " + renderer);
@@ -314,6 +331,11 @@ int main(int argc, char** argv) {
                 pp.mode = GFX_PRESENT_FLOW;
             else if (view == "cells")
                 pp.flags |= GFX_PRESENT_REGIR_CELLS;
+            else if (svgfView >= 0) {                                                     // svgf_main.cpp:1907-1911
+                pp.sourceBuffer = GFX_BUF_SVGF_DEBUG_VISUALIZE;
+                pp.sourceIndex = 0;
+                pp.flags = svgfView <= GFX_SVGF_VIEW_FILTERED_VARIANCE ? GFX_PRESENT_TONE_MAP | GFX_PRESENT_SRGB_GAMMA : 0u;
+            }
             check(gfx, gfx_present_launch(gfx, nullptr, &pp), "gfx_present_launch");
             std::vector<uint32_t> image((size_t)width * height);
             check(gfx, gfx_buffer_download(gfx, nullptr, GFX_BUF_PRESENT_RGBA8, 0, image.data(), image.size() * 4), "gfx_buffer_download");

@@ -361,7 +361,8 @@ typedef enum GfxBufferId {
     GFX_BUF_PRESAMPLED_LIGHTS = 31,     /* 12 words x 131072 : emittance3 areaPDensity | position3 atInfinity | normal3 0 */
     GFX_BUF_PRESAMPLE_RNG = 32,         /* uint64 x 131072 : lightPreSamplingRngs */
     /* output side */
-    GFX_BUF_PRESENT_RGBA8 = 33          /* uint32 per pixel, R | G << 8 | B << 16 | A << 24 : gfx_present_launch */
+    GFX_BUF_PRESENT_RGBA8 = 33,         /* uint32 per pixel, R | G << 8 | B << 16 | A << 24 : gfx_present_launch */
+    GFX_BUF_SVGF_DEBUG_VISUALIZE = 34   /* float x4 per pixel, w = 1 : gfx_svgf_debug_visualize (debugVisualizeBuffer) */
 } GfxBufferId;
 
 /* ---- context ------------------------------------------------------------------------- */
@@ -529,6 +530,33 @@ int gfx_gbuffer_launch(gfx_ctx* ctx, void* stream, const GfxFrameParams* params)
 int gfx_restir_launch(gfx_ctx* ctx, void* stream, const GfxFrameParams* params, int pass);
 /* replaces the svgf.cu kernels (svgf_main.cpp:2127-2172) */
 int gfx_svgf_launch(gfx_ctx* ctx, void* stream, const GfxFrameParams* params, int pass, uint32_t stage);
+/* The SVGF app's "Buffer to Display" debug views: debugVisualize(bufferToDisplay, motionVectorOffset, motionVectorScale,
+ * numFilteringStages) (svgf/gpu_kernels/visualize.cu:6-87).  Writes GFX_BUF_SVGF_DEBUG_VISUALIZE (allocated and zeroed on the
+ * first call; downloading it before then is refused) on the rows params->tileOriginY / tileRows, pixel (x, y) of every plane to
+ * pixel (x, y) of the view, w = 1.  The app launches Noisy Beauty and Variance after GFX_SVGF_ESTIMATE_VARIANCE and before the
+ * first a-trous stage, only with SVGF on, and the other views after GFX_SVGF_MODULATE_TAA (svgf_main.cpp:2138-2145, 2175-2185).
+ * Show the buffer with gfx_present_launch(GFX_PRESENT_COLOR): GFX_PRESENT_TONE_MAP | GFX_PRESENT_SRGB_GAMMA for Noisy Beauty,
+ * Variance and Filtered Variance, no flags for the others (:1907-1911).  Final Rendering (the app's value 7) is not a view: it
+ * is the present of GFX_BUF_SVGF_FINAL.
+ *   NOISY_BEAUTY       lighting plane 0 rgb, x the SVGF albedo with GFX_SVGF_MODULATE_ALBEDO
+ *   VARIANCE           sqrt(lighting plane 0 .w) in r, g and b
+ *   FILTERED_VARIANCE  sqrt(lighting plane numFilteringStages % 2 .w); the app passes 5 with SVGF off too, so there it shows
+ *                      plane 1 as the last frame with SVGF on left it
+ *   ALBEDO             the SVGF albedo (the thresholded DH reflectance of the temporal pass; 1 at background pixels)
+ *   NORMAL             0.5 n + 0.5 of the shading normal the temporal pass decoded.  The app reads its G-buffer, which it never
+ *                      clears (svgf_main.cpp:2036-2042), so its background pixels show stale normals; here n = 0 there, and they
+ *                      show (0.5, 0.5, 0.5).  The normal is not bump-mapped: the library has no bump mapping.
+ *   MOTION_VECTOR      mv = (W, H) * ((x + 0.5, y + 0.5) / (W, H) - prevScreenPos), the prevScreenPos of the temporal pass (hits)
+ *                      and of GFX_SVGF_FILL_BACKGROUND (background); clamp(scale * mv + offset, 0, 1) in r and g, b = offset
+ *   SAMPLE_COUNT       min(count / 255, 1), count = the low 24 bits of GFX_BUF_SVGF_MOMENTS[params->bufferIndex].z
+ * The app passes offset 0.5 and scale 10^-1 (its slider's default, :1724, 2143) and 5 stages.  A view outside 0..6:
+ * GFX_ERR_INVALID_ARGUMENT; before gfx_frame_create: GFX_ERR_NOT_READY. */
+typedef enum GfxSVGFView {            /* shared::BufferToDisplay (svgf_shared.h:247-256), same numbers */
+    GFX_SVGF_VIEW_NOISY_BEAUTY = 0, GFX_SVGF_VIEW_VARIANCE = 1, GFX_SVGF_VIEW_FILTERED_VARIANCE = 2,
+    GFX_SVGF_VIEW_ALBEDO = 3, GFX_SVGF_VIEW_NORMAL = 4, GFX_SVGF_VIEW_MOTION_VECTOR = 5, GFX_SVGF_VIEW_SAMPLE_COUNT = 6
+} GfxSVGFView;
+int gfx_svgf_debug_visualize(gfx_ctx* ctx, void* stream, const GfxFrameParams* params, int view,
+                             float motionVectorOffset, float motionVectorScale, uint32_t numFilteringStages);
 /* replaces pathTracing.setEntryPoint(variant) + pathTracing.optixPipeline.launch (path_tracing_main.cpp:1780-1789):
  * one sample per pixel of the unidirectional path tracer (NEE + MIS + Russian roulette, params->maxPathLength)
  * starting from the G-buffer of params->bufferIndex; running mean into GFX_BUFFER_BEAUTY_ACCUM. */
