@@ -315,7 +315,9 @@ GFX_D bool risPixel(const DevScene &s, const DevFrame &f, const DevFrameParams &
 }
 
 #ifndef GFX_RIS_MIN_BLOCKS
-#define GFX_RIS_MIN_BLOCKS 16 // 64 registers: occupancy over the 84 registers ptxas picks unconstrained (A/B: -DGFX_RIS_MIN_BLOCKS=...)
+// 80 registers (8 B of spills): on an H100 80GB HBM3 at a 700 W power limit the 1080p two-phase candidate pass of bench.py
+// takes 1.93 ms at 12 blocks / SM against 2.24 ms at 16 (64 registers, 136 B of spills) (A/B: -DGFX_RIS_MIN_BLOCKS=...)
+#define GFX_RIS_MIN_BLOCKS 12
 #endif
 template <bool withTemporalRIS, bool useUnbiasedEstimator, int PHASE, bool TWO_PHASE = false, bool ENV = false>
 __global__ void __launch_bounds__(64, GFX_RIS_MIN_BLOCKS) k_initialAndTemporalRIS(DevScene s, DevFrame f, DevFrameParams p) {

@@ -539,6 +539,18 @@ def tiny_city_scene() -> Scene:
                       lamp_tess=(6, 4), num_building_meshes=4, name="tiny_city")
 
 
+def tiny_city_scene_degenerate_light() -> Scene:
+    """tiny_city_scene plus a 0.5 x 0.5 quad light 10^7 units away: its object-space area gives it a few percent of the light
+    selection probability (whole buckets of the pick guide), but in world space its corners round to one line (the float
+    spacing there is 1), so its area density is infinite and its bounding sphere must never cull."""
+    scene = tiny_city_scene()
+    emitter = int(np.flatnonzero(scene.materials["hasEmittance"])[0])
+    scene.meshes.append(make_quad_light(0.5, emitter))
+    scene.instances.append(make_instance([len(scene.meshes) - 1], (1.0e7, 4.5, 0.0)))
+    scene.name = "tiny_city_degenerate_light"
+    return scene
+
+
 def load_obj(path: str):
     """Minimal OBJ reader (v / f only, fan triangulation) for data/teapot.obj-style files, plain or gzip-compressed (.gz)."""
     import gzip
