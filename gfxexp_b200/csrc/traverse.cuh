@@ -192,21 +192,29 @@ struct TraversalState {
     Hit best;
     uint32_t nodeIdx;
     int sp;
-    uint2* sstack;           // this thread's column of the shared-memory stack (wavefront kernels), else unused
-    uint2 stack[kStackSize]; // (node index, truncated entry distance bits)
+    uint2 stack[kStackSize]; // (node index, truncated entry distance bits); unused with a split stack
 };
-template <int SMEM_STRIDE> // threads per block of the shared-memory stack, 0 = local memory only
-GFX_D void stackStore(TraversalState &st, int at, const uint2 &v) {
-    if (SMEM_STRIDE > 0 && at < kSmemStack)
-        st.sstack[at * SMEM_STRIDE] = v;
+// The wavefront kernels' stack is split: `sstack` is this thread's column of the shared-memory part, `spill` a local array of
+// the kStackSize - kSmemStack deeper entries.  Both are passed along rather than kept in TraversalState.  A state whose
+// stack is indexed dynamically lives in local memory: every node step would reload the ray and the traversal position from
+// there, and a pointer loaded from there is a generic one, so every push and pop would be a generic store / load instead of
+// STS / LDS.  Without the stack the state stays in registers.
+template <int SMEM_STRIDE> // threads per block of the shared-memory stack, 0 = st.stack only
+GFX_D void stackStore(TraversalState &st, uint2* sstack, uint2* spill, int at, const uint2 &v) {
+    if (SMEM_STRIDE == 0)
+        st.stack[at] = v;
+    else if (at < kSmemStack)
+        sstack[at * SMEM_STRIDE] = v;
     else
-        st.stack[SMEM_STRIDE > 0 ? at - kSmemStack : at] = v;
+        spill[at - kSmemStack] = v;
 }
 template <int SMEM_STRIDE>
-GFX_D uint2 stackLoad(const TraversalState &st, int at) {
-    if (SMEM_STRIDE > 0 && at < kSmemStack)
-        return st.sstack[at * SMEM_STRIDE];
-    return st.stack[SMEM_STRIDE > 0 ? at - kSmemStack : at];
+GFX_D uint2 stackLoad(const TraversalState &st, const uint2* sstack, const uint2* spill, int at) {
+    if (SMEM_STRIDE == 0)
+        return st.stack[at];
+    if (at < kSmemStack)
+        return sstack[at * SMEM_STRIDE];
+    return spill[at - kSmemStack];
 }
 
 GFX_D void traverseInit(TraversalState &st, const f3 &org, const f3 &dir, float tmin, float tmax) {
@@ -230,7 +238,6 @@ GFX_D void traverseInit(TraversalState &st, const f3 &org, const f3 &dir, float 
     st.idir = f3(1.0f / sd.x, 1.0f / sd.y, 1.0f / sd.z);
     st.nodeIdx = 0;
     st.sp = 0;
-    st.sstack = nullptr;
 }
 
 // Absolute slack s of the slab distances, per axis (u = 2^-24).  traverseStep computes a slab distance as t = fmaf(q, a, b)
@@ -267,6 +274,14 @@ constexpr int kPendingLeaves = 12;
 struct PendingLeaves {
     uint32_t idx[kPendingLeaves];
     int n;
+    GFX_HD uint32_t &at(int i) { return idx[i]; }
+};
+// The same list in the wavefront kernel: `col` is this thread's column of a [kPendingLeaves][kSmemStackThreads] shared array,
+// laid out like the stack, so that the dynamically indexed entries cause no local-memory traffic.
+struct SmemPendingLeaves {
+    uint32_t* col;
+    int n;
+    GFX_HD uint32_t &at(int i) { return col[i * kSmemStackThreads]; }
 };
 
 // One triangle of a leaf chain (leaf-ordered storage).  Returns true when an any-hit ray has found its occluder.
@@ -299,18 +314,18 @@ GFX_D bool testLeafTriangle(const DevBvh &bvh, TraversalState &st, uint32_t idx,
 }
 
 // Advances the newest postponed leaf of this lane by one triangle.  Returns true when an any-hit ray is occluded.
-template <bool ANY_HIT, bool STATS>
-GFX_D bool testPendingTriangle(const DevBvh &bvh, TraversalState &st, PendingLeaves &pend) {
+template <bool ANY_HIT, bool STATS, typename Pending>
+GFX_D bool testPendingTriangle(const DevBvh &bvh, TraversalState &st, Pending &pend) {
     static_assert(ANY_HIT, "postponed leaf tests are for any-hit rays");
     const int top = pend.n - 1;
-    const uint32_t idx = pend.idx[top];
+    const uint32_t idx = pend.at(top);
     bool end;
     if (testLeafTriangle<ANY_HIT, STATS>(bvh, st, idx, &end))
         return true;
     if (end)
         pend.n = top;
     else
-        pend.idx[top] = idx + 1;
+        pend.at(top) = idx + 1;
     return false;
 }
 
@@ -328,9 +343,10 @@ GFX_D uint32_t octantOrderBits(uint32_t m, uint32_t o) {
 
 // Processes node st.nodeIdx of the traversal copy (octantOrderNode): slab-tests its children, intersects the triangle
 // chains of the leaf children that are hit (or, with `pend`, postpones them), selects the next internal node.  Returns false
-// when the traversal is finished.
-template <bool ANY_HIT, bool STATS, bool DEFER = false, int SMEM_STRIDE = 0>
-GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pend = nullptr) {
+// when the traversal is finished.  With SMEM_STRIDE > 0, the stack is split into `sstack` and `spill` (stackStore).
+template <bool ANY_HIT, bool STATS, bool DEFER = false, int SMEM_STRIDE = 0, typename Pending = PendingLeaves>
+GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, Pending* pend = nullptr, uint2* sstack = nullptr,
+                        uint2* spill = nullptr) {
     static_assert(ANY_HIT || !DEFER, "postponed leaf tests are for any-hit rays");
     const uint4* np = bvh.nodes + 5 * (size_t)st.nodeIdx;
     const uint4 n0 = __ldg(np + 0);
@@ -403,7 +419,7 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
         for (uint32_t leaves = hits & ~internalAt; leaves != 0; leaves &= leaves - 1u) {
             uint32_t idx = leafBase + GFX_META_AT(lowestBit(leaves));
             if (DEFER) {
-                pend->idx[pend->n++] = idx;
+                pend->at(pend->n++) = idx;
                 continue;
             }
             while (true) {
@@ -421,7 +437,7 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
             internals ^= 1u << p;
             if (next != 0xFFFFFFFFu) {
                 if (st.sp < kStackSize)
-                    stackStore<SMEM_STRIDE>(st, st.sp++, make_uint2(next, 0u));
+                    stackStore<SMEM_STRIDE>(st, sstack, spill, st.sp++, make_uint2(next, 0u));
                 else if (bvh.overflowFlag)
                     *bvh.overflowFlag = 1u;
             }
@@ -465,7 +481,7 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
                 continue;
             if (next != 0xFFFFFFFFu) {
                 if (st.sp < kStackSize)
-                    stackStore<SMEM_STRIDE>(st, st.sp++, make_uint2(next, nextT));
+                    stackStore<SMEM_STRIDE>(st, sstack, spill, st.sp++, make_uint2(next, nextT));
                 else if (bvh.overflowFlag)
                     *bvh.overflowFlag = 1u;
             }
@@ -479,7 +495,7 @@ GFX_D bool traverseStep(const DevBvh &bvh, TraversalState &st, PendingLeaves* pe
         return true;
     }
     while (st.sp > 0) {
-        const uint2 e = stackLoad<SMEM_STRIDE>(st, --st.sp);
+        const uint2 e = stackLoad<SMEM_STRIDE>(st, sstack, spill, --st.sp);
         if (ANY_HIT || __uint_as_float(e.y) <= st.best.dist * kRelSlack) {
             st.nodeIdx = e.x;
             return true;
@@ -496,20 +512,6 @@ GFX_D Hit traverseBvh(const DevBvh &bvh, const f3 &org, const f3 &dir, const flo
         return st.best;
     traverseSlack(st, bvh);
     while (traverseStep<ANY_HIT, STATS>(bvh, st)) {
-    }
-    return st.best;
-}
-// the same with the first kSmemStack stack entries in shared memory: `sstack` = this thread's column of a
-// [kSmemStack][STRIDE] uint2 array
-template <bool ANY_HIT, int STRIDE>
-GFX_D Hit traverseBvhSmemStack(const DevBvh &bvh, const f3 &org, const f3 &dir, const float tmin, const float tmax, uint2* sstack) {
-    TraversalState st;
-    traverseInit(st, org, dir, tmin, tmax);
-    st.sstack = sstack;
-    if (bvh.numNodes == 0)
-        return st.best;
-    traverseSlack(st, bvh);
-    while (traverseStep<ANY_HIT, false, false, STRIDE>(bvh, st)) {
     }
     return st.best;
 }

@@ -37,6 +37,7 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
     const uint32_t lane = threadIdx.x & 31u;
     __shared__ uint2 sharedStack[kSmemStack][kSmemStackThreads];
     uint2* const myStack = &sharedStack[0][threadIdx.x];
+    uint2 spillStack[kStackSize - kSmemStack];
     TraversalState st;
     bool active = false;
     uint32_t myRay = 0;
@@ -47,8 +48,8 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
     // instructions.  A lane whose traversal has ended with leaves still postponed waits
     // (`draining`) for the next flush; an occluded any-hit ray learns it at the flush.
     constexpr int kFlushLanes = GFX_TRACE_FLUSH_LANES;
-    PendingLeaves pend;
-    pend.n = 0;
+    __shared__ uint32_t sharedPending[kPendingLeaves][kSmemStackThreads];
+    SmemPendingLeaves pend{ &sharedPending[0][threadIdx.x], 0 };
     bool draining = false;
     while (true) {
         // ---- refill idle lanes (one atomic per warp)
@@ -66,7 +67,6 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
                     const float4 r1 = __ldg(rays + 2 * (size_t)r + 1);
                     traverseInit(st, f3(r0.x, r0.y, r0.z), f3(r1.x, r1.y, r1.z), r0.w, r1.w);
                     traverseSlack(st, bvh);
-                    st.sstack = myStack;
                     myRay = r;
                     active = true;
                 }
@@ -76,7 +76,7 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
             break;
 #pragma unroll 1
         for (int it = 0; it < 8; ++it) {
-            if (active && !draining && !traverseStep<ANY_HIT, STATS, true, kSmemStackThreads>(bvh, st, &pend))
+            if (active && !draining && !traverseStep<ANY_HIT, STATS, true, kSmemStackThreads>(bvh, st, &pend, myStack, spillStack))
                 draining = true;
             const uint32_t have = __ballot_sync(0xFFFFFFFFu, active && pend.n > 0);
             const uint32_t running = __ballot_sync(0xFFFFFFFFu, active && !draining);
@@ -119,7 +119,6 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
                     const float4 r1 = __ldg(rays + 2 * (size_t)r + 1);
                     traverseInit(st, f3(r0.x, r0.y, r0.z), f3(r1.x, r1.y, r1.z), r0.w, r1.w);
                     traverseSlack(st, bvh);
-                    st.sstack = myStack;
                     myRay = r;
                     active = true;
                 }
@@ -130,7 +129,8 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
         // ---- advance every active lane by up to 8 nodes, leave early once a quarter of the warp is idle
 #pragma unroll 1
         for (int it = 0; it < 8; ++it) {
-            if (active && !traverseStep<ANY_HIT, STATS, false, kSmemStackThreads>(bvh, st)) {
+            if (active && !traverseStep<ANY_HIT, STATS, false, kSmemStackThreads>(bvh, st, (PendingLeaves*)nullptr, myStack,
+                                                                               spillStack)) {
                 writer.template write<ANY_HIT, STATS>(myRay, st);
                 active = false;
             }
@@ -160,8 +160,9 @@ static inline int wavefrontGrid() {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    // 9 x 128 threads per SM: what 56 registers admit; GFX_TRACE_BLOCKS_PER_SM overrides (A/B)
-    static const int perSm = [] { const char* e = getenv("GFX_TRACE_BLOCKS_PER_SM"); const int v = e ? atoi(e) : 0; return v > 0 && v <= 32 ? v : 9; }();
+    // 8 x 128 threads per SM: what the any-hit kernels' 64 registers admit (H100, visibility tracer: 0.78 ms per launch at 8
+    // and at 9, 0.81 at 7; capping them at 56 registers for 9 blocks spills and costs 0.84); GFX_TRACE_BLOCKS_PER_SM overrides (A/B)
+    static const int perSm = [] { const char* e = getenv("GFX_TRACE_BLOCKS_PER_SM"); const int v = e ? atoi(e) : 0; return v > 0 && v <= 32 ? v : 8; }();
     return sms * perSm;
 }
 
