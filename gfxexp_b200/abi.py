@@ -45,7 +45,12 @@ class GfxSceneDesc(C.Structure):
                 ("numMeshes", c_u32), ("numMaterials", c_u32), ("numInstances", c_u32),
                 ("numInstanceMeshSlots", c_u32),
                 ("envTexels", C.POINTER(c_f)), ("envWidth", c_u32), ("envHeight", c_u32),
-                ("textures", C.POINTER(GfxTextureDesc)), ("materialTextures", C.POINTER(c_u32)), ("numTextures", c_u32)]
+                ("textures", C.POINTER(GfxTextureDesc)), ("materialTextures", C.POINTER(c_u32)), ("numTextures", c_u32),
+                ("bumpMaps", C.POINTER(c_u32))]
+
+
+BUMP_NORMAL_MAP, BUMP_HEIGHT_MAP = 0, 1  # GfxBumpMapType
+NO_BUMP_MAP = 0xFFFFFFFF                 # bumpMaps[2 m]: the reference's default 1x1 texel
 
 
 class GfxBvhInfo(C.Structure):
@@ -77,7 +82,8 @@ class GfxFrameParams(C.Structure):
                 ("regirLog2NumCandidatesPerCell", c_u32), ("regirEnableCellRandomization", c_u32),
                 ("reuseVisibilityForTemporal", c_u32), ("reuseVisibilityForSpatiotemporal", c_u32),
                 ("radiusThresholdForSpatialVisReuse", c_f),
-                ("enableEnvLight", c_u32), ("envLightPowerCoeff", c_f), ("envLightRotation", c_f)]
+                ("enableEnvLight", c_u32), ("envLightPowerCoeff", c_f), ("envLightRotation", c_f),
+                ("enableBumpMapping", c_u32)]
 
 
 class GfxPresentParams(C.Structure):
@@ -207,11 +213,17 @@ class SceneArrays:
                 assert t.ndim == 3 and t.shape[2] == 4
                 d.texels = t.ctypes.data_as(C.POINTER(c_f))
                 d.height, d.width = t.shape[0], t.shape[1]
-            self.material_textures = np.ascontiguousarray(scene.material_textures, dtype=np.uint32).reshape(-1, 4)
-            assert self.material_textures.shape[0] == mats.shape[0]
             self.desc.textures = C.cast(self.texture_descs, C.POINTER(GfxTextureDesc))
-            self.desc.materialTextures = self.material_textures.ctypes.data_as(C.POINTER(c_u32))
             self.desc.numTextures = len(self.textures)
+            if scene.material_textures is not None:  # None: the textures are bump maps only
+                self.material_textures = np.ascontiguousarray(scene.material_textures, dtype=np.uint32).reshape(-1, 4)
+                assert self.material_textures.shape[0] == mats.shape[0]
+                self.desc.materialTextures = self.material_textures.ctypes.data_as(C.POINTER(c_u32))
+        bump_maps = getattr(scene, "bump_maps", None)  # uint32 [numMaterials, 2]: texture index or NO_BUMP_MAP, GfxBumpMapType
+        if bump_maps is not None:
+            self.bump_maps = np.ascontiguousarray(bump_maps, dtype=np.uint32).reshape(-1, 2)
+            assert self.bump_maps.shape[0] == mats.shape[0]
+            self.desc.bumpMaps = self.bump_maps.ctypes.data_as(C.POINTER(c_u32))
 
 
 def make_instance_descs(instances):
@@ -278,6 +290,7 @@ def default_frame_params(scene, width: int, height: int) -> GfxFrameParams:
     p.reuseVisibilityForTemporal = 1
     p.reuseVisibilityForSpatiotemporal = 0
     p.radiusThresholdForSpatialVisReuse = 10.0
+    p.enableBumpMapping = 0  # perFramePlp.enableBumpMapping = false in every app (restir_di_main.cpp:1986)
     return p
 
 
@@ -383,6 +396,7 @@ _DECLS = {
     "gfx_launch_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GfxBatchOp), c_u32]),
     "gfx_light_pick_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, c_u32, C.c_void_p, C.c_void_p]),
     "gfx_env_light_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, c_u32, C.c_void_p]),
+    "gfx_bump_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, c_u32, C.c_void_p, c_u32, C.c_void_p]),
     "gfx_light_dist_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_f)]),
     "gfx_frame_create": (C.c_int, [C.c_void_p, c_u32, c_u32]),
     "gfx_rng_seed": (C.c_int, [C.c_void_p, C.c_uint64]),

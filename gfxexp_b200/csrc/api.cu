@@ -15,7 +15,7 @@ void SceneState::release() {
     cudaFree(primWeights); cudaFree(primCdf); cudaFree(geomWeights); cudaFree(geomCdf);
     cudaFree(instWeights); cudaFree(instCdf); cudaFree(instIntegral);
     cudaFree(primProb); cudaFree(geomProb); cudaFree(instProb); cudaFree(lightTris); cudaFree(lightTriBase); cudaFree(emissiveGeoms); cudaFree(instGuide); cudaFree(primGuide);
-    cudaFree(texPool); cudaFree(texTable); cudaFree(materialTextures);
+    cudaFree(texPool); cudaFree(texTable); cudaFree(materialTextures); cudaFree(bumpTable); cudaFree(bumpDefaultTexel);
     cudaFree(envTexels); cudaFree(envPdf); cudaFree(envCdf); cudaFree(envTopPdf); cudaFree(envTopCdf);
     cudaFree(pickGuide); cudaFree(normalMats); cudaFree(pickPieces); cudaFree(pickKeyAt); cudaFree(pickBoundaries); cudaFree(pickCounters); cudaFree(pickSortTemp);
     if (pickFlagsHost) cudaFreeHost(pickFlagsHost);
@@ -186,6 +186,8 @@ DevScene gfx_ctx::devScene() const {
     d.texPool = scene.texPool;
     d.texTable = scene.texTable;
     d.materialTextures = scene.materialTextures;
+    d.bumpTable = scene.bumpTable;
+    d.bumpTexels = scene.bumpTexels;
     d.env.texels = scene.envTexels;
     d.env.pdf = scene.envPdf;
     d.env.cdf = scene.envCdf;
@@ -729,6 +731,15 @@ int gfx_env_light_debug(gfx_ctx* ctx, void* stream, int op, const float* in, uin
     if ((n && (!in || !out)) || op < 0 || op > 2)
         return GFX_ERR_INVALID_ARGUMENT;
     return debugEnvLight(ctx, (cudaStream_t)stream, op, in, n, out);
+}
+
+int gfx_bump_debug(gfx_ctx* ctx, void* stream, int op, uint32_t matSlot, const float* in, uint32_t n, float* out) {
+    CHECK_CTX(ctx);
+    if (!ctx->scene.uploaded)
+        return GFX_ERR_NOT_READY;
+    if ((n && (!in || !out)) || op < 0 || op > 2 || (op != 1 && matSlot >= ctx->scene.numMaterials))
+        return GFX_ERR_INVALID_ARGUMENT;
+    return debugBump(ctx, (cudaStream_t)stream, op, matSlot, in, n, out);
 }
 
 int gfx_light_dist_export(gfx_ctx* ctx, float* instWeights, float* instCdf, float* integral) {

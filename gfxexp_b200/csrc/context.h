@@ -45,6 +45,9 @@ struct SceneState {
     float4* texPool = nullptr;
     uint4* texTable = nullptr;
     uint4* materialTextures = nullptr;
+    uint4* bumpTable = nullptr;            // per material, see DevScene::bumpTable
+    float4* bumpTexels = nullptr;          // texPool, or bumpDefaultTexel for a scene without bump maps (not owned)
+    float4* bumpDefaultTexel = nullptr;
     // environment light (lights.cu uploadEnvLight): texels + the importance map's distributions
     float4* envTexels = nullptr;
     float* envPdf = nullptr;
@@ -275,6 +278,8 @@ int buildLightDistributions(gfx_ctx* ctx, cudaStream_t stream, uint32_t bufferIn
 int uploadEnvLight(gfx_ctx* ctx, const float* rgba, uint32_t width, uint32_t height);
 int uploadTextures(gfx_ctx* ctx, const GfxSceneDesc* sd);
 int debugEnvLight(gfx_ctx* ctx, cudaStream_t stream, int op, const float* dIn, uint32_t n, float* dOut);
+int ensureBumpTable(gfx_ctx* ctx); // lights.cu, before a launch with enableBumpMapping
+int debugBump(gfx_ctx* ctx, cudaStream_t stream, int op, uint32_t matSlot, const float* dIn, uint32_t n, float* dOut);
 int debugLightPick(gfx_ctx* ctx, cudaStream_t stream, const float* dUl, uint32_t n, uint32_t* dFlat, uint32_t* dChain);
 size_t lightPickSortTempBytes(uint32_t capacity);
 int launchGBuffer(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p);

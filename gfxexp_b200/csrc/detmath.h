@@ -157,6 +157,14 @@ DM_HD float dm_atan_pos(float x) {
     return y + p;
 }
 
+// atan(x) for every x: odd extension of dm_atan_pos (the sign bit is kept, so atan(-0) = -0; +-inf -> +-pi/2, NaN -> NaN).
+// applyBumpMapping's tiltAngle = atan(projLength / z) (common_device.cuh:184), where z may be 0 or negative.
+DM_HD float dm_atan(float x) {
+    if (x != x) return x;
+    const float a = dm_atan_pos(fabsf(x));
+    return (dm_f2u(x) >> 31) ? -a : a;
+}
+
 // atan2(y, x) in [-pi, pi].
 DM_HD float dm_atan2(float y, float x) {
     if (x == 0.0f) {

@@ -31,8 +31,9 @@ GFX_D void countRays(const DevFrame &frame, uint32_t n) {
         atomicAdd(frame.stats, (unsigned long long)total);
 }
 
-// JITTER: GFX_SVGF_SUBPIXEL_JITTER, the primary ray through (x, y) + sample (svgfSubPixelSample) and no random number drawn
-template <bool JITTER>
+// JITTER: GFX_SVGF_SUBPIXEL_JITTER, the primary ray through (x, y) + sample (svgfSubPixelSample) and no random number drawn.
+// BUMP: GfxFrameParams::enableBumpMapping, a kernel of its own so that the frames without it run the code they ran before it existed
+template <bool JITTER, bool BUMP>
 GFX_D uint32_t gbufferPixel(const DevScene &scene, const DevFrame &frame, const DevFrameParams &p, float2 sample) {
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
     const uint32_t y = p.y0 + blockIdx.y * 8 + threadIdx.y;
@@ -112,7 +113,9 @@ GFX_D uint32_t gbufferPixel(const DevScene &scene, const DevFrame &frame, const 
         qTexCoord = encodeTexCoords(texCoord);
 
         const BSDF bsdf = setupBsdf(scene, matSlot, texCoord);
-        const ReferenceFrame shadingFrame(shadingNormalInWorld, texCoord0DirInWorld);
+        ReferenceFrame shadingFrame(shadingNormalInWorld, texCoord0DirInWorld);
+        if (BUMP) // optix_gbuffer_kernels.cu:175-178 (restir_di, regir), :151-154 (path_tracing, NRC)
+            shadingFrame = bumpShadingFrame(scene, matSlot, texCoord, shadingFrame);
         const f3 vOut = -direction;
         const f3 vOutLocal = shadingFrame.toLocal(normalize(vOut));
         shadingNormalInWorld = shadingFrame.normal;
@@ -169,18 +172,22 @@ GFX_D uint32_t gbufferPixel(const DevScene &scene, const DevFrame &frame, const 
     return 1;
 }
 
+template <bool BUMP>
 __global__ void __launch_bounds__(64) k_gbuffer(DevScene scene, DevFrame frame, DevFrameParams p) {
-    countRays(frame, gbufferPixel<false>(scene, frame, p, make_float2(0.5f, 0.5f)));
+    countRays(frame, gbufferPixel<false, BUMP>(scene, frame, p, make_float2(0.5f, 0.5f)));
 }
 
+template <bool BUMP>
 __global__ void __launch_bounds__(64) k_gbufferSubPixelJitter(DevScene scene, DevFrame frame, DevFrameParams p, float2 sample) {
-    countRays(frame, gbufferPixel<true>(scene, frame, p, sample));
+    countRays(frame, gbufferPixel<true, BUMP>(scene, frame, p, sample));
 }
 
 int launchGBuffer(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params) {
     bool jitter;
     float2 sample;
-    const int rc = svgfSubPixelSample(ctx, params, &jitter, &sample);
+    int rc = svgfSubPixelSample(ctx, params, &jitter, &sample);
+    if (rc == GFX_OK && params->enableBumpMapping)
+        rc = ensureBumpTable(ctx);
     if (rc != GFX_OK)
         return rc;
     const DevFrameParams p = makeDevParams(ctx, params);
@@ -189,10 +196,15 @@ int launchGBuffer(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* param
     const dim3 block(8, 8);
     const dim3 grid((ctx->frame.W + 7) / 8, (p.y1 - p.y0 + 7) / 8);
     GFX_TIMED(ctx, stream, "gbuffer");
-    if (jitter)
-        k_gbufferSubPixelJitter<<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p, sample);
+    const bool bump = params->enableBumpMapping != 0;
+    if (jitter && bump)
+        k_gbufferSubPixelJitter<true><<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p, sample);
+    else if (jitter)
+        k_gbufferSubPixelJitter<false><<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p, sample);
+    else if (bump)
+        k_gbuffer<true><<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p);
     else
-        k_gbuffer<<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p);
+        k_gbuffer<false><<<grid, block, 0, stream>>>(ctx->devScene(), ctx->devFrame(), p);
     ctx->launches++;
     GFX_CUDA(ctx, cudaGetLastError());
     return GFX_OK;

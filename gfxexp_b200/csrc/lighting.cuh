@@ -612,4 +612,70 @@ GFX_D BSDF setupBsdf(const DevScene &s, uint32_t matSlot, const f2 &texCoord) {
     return b;
 }
 
+// ---- bump mapping (perFramePlp.enableBumpMapping) ------------------------------------------------------------------------
+// tex2Dgather<float4>(texture, u, v, 0) with repeat addressing in software: channel 0 of the 2x2 footprint of the linear filter
+// (xB = frac(u) W - 0.5, i0 = floor(xB), i1 = i0 + 1, both wrapped; likewise j0, j1 in v), in the order of the PTX ISA's tld4
+// ("Texture Instructions: tld4"): x = (i0, j1), y = (i1, j1), z = (i1, j0), w = (i0, j0).  The texture unit keeps the position
+// with 8 fractional bits: a fraction above 255.5 / 256 moves the footprint one texel on.  tests/test_gpu_bump.py checks this against
+// tld4; only within about 0.01 / 256 texel of that boundary does the unit's own fixed-point position decide otherwise.
+GFX_D uint32_t gatherIndex(float xB, uint32_t W) {
+    const float fx = floorf(xB);
+    const int ix = dm_f2int(fx) + ((xB - fx) * 256.0f > 255.5f ? 1 : 0); // -1 .. W
+    return ix < 0 ? W - 1 : ((uint32_t)ix >= W ? (uint32_t)ix - W : (uint32_t)ix);
+}
+GFX_D float4 textureGatherRepeat(const float4* texels, uint32_t W, uint32_t H, float u, float v) {
+    const uint32_t x0 = gatherIndex((u - floorf(u)) * W - 0.5f, W), y0 = gatherIndex((v - floorf(v)) * H - 0.5f, H);
+    const uint32_t x1 = x0 + 1 >= W ? 0u : x0 + 1, y1 = y0 + 1 >= H ? 0u : y0 + 1;
+    return make_float4(__ldg(&texels[(size_t)y1 * W + x0].x), __ldg(&texels[(size_t)y1 * W + x1].x),
+                       __ldg(&texels[(size_t)y0 * W + x1].x), __ldg(&texels[(size_t)y0 * W + x0].x));
+}
+// MaterialData::readModifiedNormal(mat.normal, mat.normalDimInfo, texCoord, 0.0f) (common_device.cuh:205-240): the tangent-frame
+// normal of a normal map (:205-213, sample<float4> = tex2DLod at level 0, :143-147; y flipped: calcDimInfo's isLeftHanded = true,
+// common_host.cpp:1440-1451, 1543) or of a height map (:227-238)
+GFX_D f3 readModifiedNormal(const float4* texels, uint32_t W, uint32_t H, uint32_t type, float u, float v) {
+    if (type == GFX_BUMP_HEIGHT_MAP) {
+        const float4 heightValues = textureGatherRepeat(texels, W, H, u, v);
+        const float coeff = 5.0f / 1024;
+        const float dhdu = (coeff * W) * (heightValues.y - heightValues.x);
+        const float dhdv = (coeff * H) * (heightValues.x - heightValues.w);
+        return normalize(f3(-dhdu, dhdv, 1));
+    }
+    const float4 texValue = textureFetchRepeat(texels, W, H, u, v);
+    f3 modLocalNormal(texValue.x, texValue.y, texValue.z);
+    modLocalNormal = 2.0f * modLocalNormal - f3(1.0f);
+    modLocalNormal.y *= -1;
+    return modLocalNormal;
+}
+// applyBumpMapping (common_device.cuh:176-203): the frame rotated by the quaternion that takes (0, 0, 1) to the modified normal;
+// atan of the quotient (not atan2: z <= 0 tilts the other way), and the normal is matTFtoW * modNormalInTF, not renormalised
+GFX_D ReferenceFrame applyBumpMapping(const f3 &modNormalInTF, const ReferenceFrame &frameToModify) {
+    const float projLength = sqrtf(modNormalInTF.x * modNormalInTF.x + modNormalInTF.y * modNormalInTF.y);
+    if (projLength < 1e-3f)
+        return frameToModify;
+    const float tiltAngle = dm_atan(projLength / modNormalInTF.z);
+    float qSin, qCos;
+    dm_sincos(tiltAngle / 2, &qSin, &qCos);
+    const float qX = (-modNormalInTF.y / projLength) * qSin;
+    const float qY = (modNormalInTF.x / projLength) * qSin;
+    const float qW = qCos;
+    const f3 modTangentInTF(1 - 2 * qY * qY, 2 * qX * qY, -2 * qY * qW);
+    const f3 modBitangentInTF(2 * qX * qY, 1 - 2 * qX * qX, 2 * qX * qW);
+    // Matrix3x3(tangent, bitangent, normal) * v: row i dotted with v, i.e. fromLocal
+    ReferenceFrame bumpShadingFrame;
+    bumpShadingFrame.tangent = frameToModify.fromLocal(modTangentInTF);
+    bumpShadingFrame.bitangent = frameToModify.fromLocal(modBitangentInTF);
+    bumpShadingFrame.normal = frameToModify.fromLocal(modNormalInTF);
+    return bumpShadingFrame;
+}
+// The bump of a shading frame, out of line; only the kernels' BUMP variants (selected on the host from enableBumpMapping) call it,
+// so that a frame without bump mapping runs the code it ran before the switch existed.
+static __device__ __noinline__ ReferenceFrame bumpShadingFrameOutOfLine(const uint4* bumpTable, const float4* bumpTexels, uint32_t matSlot,
+                                                                        float tu, float tv, ReferenceFrame frame) {
+    const uint4 b = __ldg(bumpTable + matSlot);
+    return applyBumpMapping(readModifiedNormal(bumpTexels + b.x, b.y, b.z, b.w, tu, tv), frame);
+}
+GFX_D ReferenceFrame bumpShadingFrame(const DevScene &s, uint32_t matSlot, const f2 &texCoord, const ReferenceFrame &frame) {
+    return bumpShadingFrameOutOfLine(s.bumpTable, s.bumpTexels, matSlot, texCoord.x, texCoord.y, frame);
+}
+
 } // namespace gfx

@@ -571,16 +571,24 @@ int uploadEnvLight(gfx_ctx* ctx, const float* rgba, uint32_t width, uint32_t hei
     return GFX_OK;
 }
 
-// image textures of the materials: one pool of texels, a table of (offset, width, height) and the per-material indices
+// createNormalTexture without a file (common_host.cpp:1396-1412): createImmTexture's UNORM8 of (0.5, 0.5, 1), i.e. 127, 127, 255
+static const float4 kDefaultBumpTexel = make_float4(127.0f / 255.0f, 127.0f / 255.0f, 1.0f, 1.0f);
+
+// image textures of the materials: one pool of texels, a table of (offset, width, height) and the per-material indices.  With
+// bump maps also their table (offset, width, height, type) per material, whose default entry is a 1x1 texel at the end of the
+// pool; a scene without bump maps allocates exactly what it did before they existed (ensureBumpTable adds the table when a
+// frame first asks for bump mapping).
 int uploadTextures(gfx_ctx* ctx, const GfxSceneDesc* sd) {
     SceneState &S = ctx->scene;
-    if (!sd->materialTextures || !sd->numTextures)
+    const bool colourMaps = sd->materialTextures && sd->numTextures;
+    const uint32_t numTextures = (colourMaps || sd->bumpMaps) ? sd->numTextures : 0u;
+    if (!colourMaps && !sd->bumpMaps)
         return GFX_OK;
-    if (!sd->textures)
+    if (numTextures && !sd->textures)
         return GFX_ERR_INVALID_ARGUMENT;
-    std::vector<uint4> table(sd->numTextures);
+    std::vector<uint4> table(numTextures);
     size_t total = 0;
-    for (uint32_t t = 0; t < sd->numTextures; ++t) {
+    for (uint32_t t = 0; t < numTextures; ++t) {
         const GfxTextureDesc &d = sd->textures[t];
         if (!d.texels || !d.width || !d.height || total + (size_t)d.width * d.height > 0xFFFFFFFFull) {
             ctx->setError("gfx_scene_upload: empty or oversized texture");
@@ -589,8 +597,8 @@ int uploadTextures(gfx_ctx* ctx, const GfxSceneDesc* sd) {
         table[t] = make_uint4((uint32_t)total, d.width, d.height, 0u);
         total += (size_t)d.width * d.height;
     }
-    std::vector<uint4> perMaterial(sd->numMaterials);
-    for (uint32_t m = 0; m < sd->numMaterials; ++m) {
+    std::vector<uint4> perMaterial(colourMaps ? sd->numMaterials : 0u);
+    for (uint32_t m = 0; m < perMaterial.size(); ++m) {
         const uint32_t* k = sd->materialTextures + 4 * (size_t)m;
         for (int c = 0; c < 4; ++c)
             if (k[c] != 0xFFFFFFFFu && k[c] >= sd->numTextures) {
@@ -603,9 +611,28 @@ int uploadTextures(gfx_ctx* ctx, const GfxSceneDesc* sd) {
         }
         perMaterial[m] = make_uint4(k[0], k[1], k[2], k[3]);
     }
-    GFX_CUDA(ctx, cudaMalloc((void**)&S.texPool, total * 16));
-    for (uint32_t t = 0; t < sd->numTextures; ++t)
+    const uint32_t defaultTexel = (uint32_t)total;
+    std::vector<uint4> bump(sd->numMaterials ? sd->numMaterials : 1u, make_uint4(defaultTexel, 1u, 1u, GFX_BUMP_NORMAL_MAP));
+    for (uint32_t m = 0; sd->bumpMaps && m < sd->numMaterials; ++m) {
+        const uint32_t idx = sd->bumpMaps[2 * (size_t)m], type = sd->bumpMaps[2 * (size_t)m + 1];
+        if ((idx != 0xFFFFFFFFu && idx >= numTextures) || (type != GFX_BUMP_NORMAL_MAP && type != GFX_BUMP_HEIGHT_MAP)) {
+            ctx->setError("gfx_scene_upload: bump map index out of range or unknown GfxBumpMapType");
+            return GFX_ERR_INVALID_ARGUMENT;
+        }
+        if (idx != 0xFFFFFFFFu)
+            bump[m] = make_uint4(table[idx].x, table[idx].y, table[idx].z, type);
+    }
+    GFX_CUDA(ctx, cudaMalloc((void**)&S.texPool, (total + (sd->bumpMaps ? 1 : 0)) * 16));
+    for (uint32_t t = 0; t < numTextures; ++t)
         GFX_CUDA(ctx, cudaMemcpy(S.texPool + table[t].x, sd->textures[t].texels, (size_t)table[t].y * table[t].z * 16, cudaMemcpyHostToDevice));
+    if (sd->bumpMaps) {
+        GFX_CUDA(ctx, cudaMemcpy(S.texPool + defaultTexel, &kDefaultBumpTexel, 16, cudaMemcpyHostToDevice));
+        GFX_CUDA(ctx, cudaMalloc((void**)&S.bumpTable, bump.size() * 16));
+        GFX_CUDA(ctx, cudaMemcpy(S.bumpTable, bump.data(), bump.size() * 16, cudaMemcpyHostToDevice));
+        S.bumpTexels = S.texPool;
+    }
+    if (!colourMaps)
+        return GFX_OK;
     GFX_CUDA(ctx, cudaMalloc((void**)&S.texTable, table.size() * 16));
     GFX_CUDA(ctx, cudaMemcpy(S.texTable, table.data(), table.size() * 16, cudaMemcpyHostToDevice));
     GFX_CUDA(ctx, cudaMalloc((void**)&S.materialTextures, perMaterial.size() * 16));
@@ -642,6 +669,108 @@ int debugEnvLight(gfx_ctx* ctx, cudaStream_t stream, int op, const float* dIn, u
         k_envDebug<<<(n + 127) / 128, 128, 0, stream>>>(s.env, op, reinterpret_cast<const float2*>(dIn), n, dOut);
     ctx->launches++;
     GFX_CUDA(ctx, cudaGetLastError());
+    return GFX_OK;
+}
+
+// a scene uploaded without bump maps: every material reads the default texel, from a table made the first time a frame enables
+// bump mapping (allocated then, so that the switch-off frames keep the memory layout of a build without bump mapping)
+int ensureBumpTable(gfx_ctx* ctx) {
+    SceneState &S = ctx->scene;
+    if (S.bumpTable)
+        return GFX_OK;
+    const std::vector<uint4> bump(S.numMaterials ? S.numMaterials : 1u, make_uint4(0u, 1u, 1u, GFX_BUMP_NORMAL_MAP));
+    GFX_CUDA(ctx, cudaMalloc((void**)&S.bumpDefaultTexel, 16));
+    GFX_CUDA(ctx, cudaMemcpy(S.bumpDefaultTexel, &kDefaultBumpTexel, 16, cudaMemcpyHostToDevice));
+    GFX_CUDA(ctx, cudaMalloc((void**)&S.bumpTable, bump.size() * 16));
+    GFX_CUDA(ctx, cudaMemcpy(S.bumpTable, bump.data(), bump.size() * 16, cudaMemcpyHostToDevice));
+    S.bumpTexels = S.bumpDefaultTexel;
+    return GFX_OK;
+}
+
+// test hook (gfx_bump_debug): readModifiedNormal, applyBumpMapping, and the software gather next to the texture unit's
+__global__ void k_bumpDebug(DevScene s, int op, uint4 bump, cudaTextureObject_t hwTex, const float* in, uint32_t n, float* out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    if (op == 1) {
+        const float* a = in + 12 * (size_t)i;
+        ReferenceFrame frame;
+        frame.tangent = f3(a[3], a[4], a[5]);
+        frame.bitangent = f3(a[6], a[7], a[8]);
+        frame.normal = f3(a[9], a[10], a[11]);
+        const ReferenceFrame r = applyBumpMapping(f3(a[0], a[1], a[2]), frame);
+        float* o = out + 9 * (size_t)i;
+        o[0] = r.tangent.x; o[1] = r.tangent.y; o[2] = r.tangent.z;
+        o[3] = r.bitangent.x; o[4] = r.bitangent.y; o[5] = r.bitangent.z;
+        o[6] = r.normal.x; o[7] = r.normal.y; o[8] = r.normal.z;
+        return;
+    }
+    const float u = in[2 * (size_t)i], v = in[2 * (size_t)i + 1];
+    if (op == 0) {
+        const f3 m = readModifiedNormal(s.bumpTexels + bump.x, bump.y, bump.z, bump.w, u, v);
+        float* o = out + 3 * (size_t)i;
+        o[0] = m.x; o[1] = m.y; o[2] = m.z;
+        return;
+    }
+    const float4 sw = textureGatherRepeat(s.bumpTexels + bump.x, bump.y, bump.z, u, v);
+    const float4 hw = tex2Dgather<float4>(hwTex, u, v, 0);
+    float* o = out + 8 * (size_t)i;
+    o[0] = sw.x; o[1] = sw.y; o[2] = sw.z; o[3] = sw.w;
+    o[4] = hw.x; o[5] = hw.y; o[6] = hw.z; o[7] = hw.w;
+}
+int debugBump(gfx_ctx* ctx, cudaStream_t stream, int op, uint32_t matSlot, const float* dIn, uint32_t n, float* dOut) {
+    const int rc = ensureBumpTable(ctx);
+    if (rc != GFX_OK)
+        return rc;
+    const DevScene s = ctx->devScene();
+    uint4 bump = make_uint4(0, 0, 0, 0);
+    if (op != 1)
+        GFX_CUDA(ctx, cudaMemcpy(&bump, s.bumpTable + matSlot, 16, cudaMemcpyDeviceToHost));
+    cudaArray_t array = nullptr;
+    cudaTextureObject_t tex = 0;
+    auto release = [&]() {
+        if (tex)
+            cudaDestroyTextureObject(tex);
+        if (array)
+            cudaFreeArray(array);
+    };
+    if (op == 2) {
+        // the map as the reference holds it: UNORM8 RGBA in a cudaArray read through a texture object with sampler_normFloat
+        // (common_host.cpp:1476-1481: normalised float, linear filter, repeat addressing, normalised coordinates)
+        std::vector<float4> texels((size_t)bump.y * bump.z);
+        GFX_CUDA(ctx, cudaMemcpy(texels.data(), s.bumpTexels + bump.x, texels.size() * 16, cudaMemcpyDeviceToHost));
+        std::vector<uchar4> q(texels.size());
+        auto unorm8 = [](float x) { return (unsigned char)std::lround(std::fmin(std::fmax(x, 0.0f), 1.0f) * 255.0f); };
+        for (size_t k = 0; k < texels.size(); ++k)
+            q[k] = make_uchar4(unorm8(texels[k].x), unorm8(texels[k].y), unorm8(texels[k].z), unorm8(texels[k].w));
+        const cudaChannelFormatDesc fmt = cudaCreateChannelDesc<uchar4>();
+        cudaError_t e = cudaMallocArray(&array, &fmt, bump.y, bump.z);
+        if (e == cudaSuccess)
+            e = cudaMemcpy2DToArray(array, 0, 0, q.data(), (size_t)bump.y * 4, (size_t)bump.y * 4, bump.z, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) {
+            cudaResourceDesc res = {};
+            res.resType = cudaResourceTypeArray;
+            res.res.array.array = array;
+            cudaTextureDesc td = {};
+            td.addressMode[0] = td.addressMode[1] = cudaAddressModeWrap;
+            td.filterMode = cudaFilterModeLinear;
+            td.readMode = cudaReadModeNormalizedFloat;
+            td.normalizedCoords = 1;
+            e = cudaCreateTextureObject(&tex, &res, &td, nullptr);
+        }
+        if (e != cudaSuccess) {
+            release();
+            GFX_CUDA(ctx, e);
+        }
+    }
+    if (n)
+        k_bumpDebug<<<(n + 127) / 128, 128, 0, stream>>>(s, op, bump, tex, dIn, n, dOut);
+    ctx->launches++;
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess && op == 2)
+        e = cudaStreamSynchronize(stream); // the texture object must outlive the kernel
+    release();
+    GFX_CUDA(ctx, e);
     return GFX_OK;
 }
 

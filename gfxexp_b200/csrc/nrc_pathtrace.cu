@@ -284,7 +284,10 @@ GFX_D void emitRaysNrc(const DevScene &s, const DevPathState &ps, const DevNrc &
         atomicAdd(s.rayCounter, (unsigned long long)cnt);
 }
 
-// pathTrace_raygen_generic<true> up to the path extension loop (optix_pathtracing_kernels.cu:95-283)
+// pathTrace_raygen_generic<true> up to the path extension loop (optix_pathtracing_kernels.cu:95-283).  BUMP:
+// GfxFrameParams::enableBumpMapping (a kernel of its own, so that the frames without it run the code they ran before it existed;
+// likewise k_nrcBounce and k_nrcVisualizeQueries)
+template <bool BUMP>
 __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, DevNrc n) {
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
     const uint32_t y = p.y0 + blockIdx.y * 8 + threadIdx.y;
@@ -336,7 +339,9 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrame
             const float frontHit = primaryDotVN >= 0.0f ? 1.0f : -1.0f;
             positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
             primaryPathSpread = primaryDist2 / (4 * kPi * fabsf(primaryDotVN));
-            const ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+            ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+            if (BUMP) // :182-185
+                shadingFrame = bumpShadingFrameAtHit(s, mesh, gb0.z, bcB, bcC, shadingFrame);
             const f3 vOutLocal = shadingFrame.toLocal(vOut);
 
             radiance = f3(0.0f);
@@ -364,6 +369,7 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrame
 }
 
 // pathTrace_closestHit_generic<true> (:363-623) + the loop bookkeeping (:285-311) on the queue of live paths
+template <bool BUMP>
 __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, DevNrc n, uint32_t round) {
     const uint32_t curQueue = round & 1u, nextQueue = curQueue ^ 1u;
     const uint32_t* roundCounters = ps.counters + 4 * round;
@@ -442,7 +448,9 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
 
                 const f3 vOut = normalize(-rayDir);
                 const float frontHit = dot(vOut, sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
-                const ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+                ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+                if (BUMP) // :398-401
+                    shadingFrame = bumpShadingFrameAtHit(s, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), shadingFrame);
                 positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
                 const f3 vOutLocal = shadingFrame.toLocal(vOut);
 
@@ -765,7 +773,12 @@ int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* 
             ctx->launches++;
         }
     };
-    { GFX_TIMED(ctx, stream, "nrc_first_hit"); k_nrcFirstHit<<<grid, block, 0, stream>>>(s, f, p, ps, n); }
+    const bool bump = params->enableBumpMapping != 0;
+    { GFX_TIMED(ctx, stream, "nrc_first_hit");
+    if (bump)
+        k_nrcFirstHit<true><<<grid, block, 0, stream>>>(s, f, p, ps, n);
+    else
+        k_nrcFirstHit<false><<<grid, block, 0, stream>>>(s, f, p, ps, n); }
     commit();
     ctx->launches += 1;
     const int traceGrid = wavefrontGrid();
@@ -777,7 +790,11 @@ int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* 
         uint32_t* c = F.ptCounters + 4 * round;
         { GFX_TIMED(ctx, stream, "nrc_trace_shadow"); k_traceWavefront<true, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.shadowRays, c + 2, 0u, c + 3, shadowWriter); }
         { GFX_TIMED(ctx, stream, "nrc_trace_extension"); k_traceWavefront<false, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.extRays[round & 1], c + 0, 0u, c + 1, extWriter); }
-        { GFX_TIMED(ctx, stream, "nrc_bounce"); k_nrcBounce<<<sms * 16, 64, 0, stream>>>(s, f, p, ps, n, round); }
+        { GFX_TIMED(ctx, stream, "nrc_bounce");
+        if (bump)
+            k_nrcBounce<true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, n, round);
+        else
+            k_nrcBounce<false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, n, round); }
         commit();
         ctx->launches += 3;
     }
@@ -802,6 +819,7 @@ int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* 
 // ---------------------------------------------------------------------------------------------------------
 // visualizePrediction (optix_pathtracing_kernels.cu:702-778): the primary hit's radiance query, as k_nrcFirstHit builds it,
 // at row y * W + x; a miss leaves its row untouched
+template <bool BUMP>
 __global__ void __launch_bounds__(64) k_nrcVisualizeQueries(DevScene s, DevFrame f, DevFrameParams p, DevNrc n) {
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
     const uint32_t y = blockIdx.y * 8 + threadIdx.y;
@@ -825,7 +843,9 @@ __global__ void __launch_bounds__(64) k_nrcVisualizeQueries(DevScene s, DevFrame
         const float primaryDotVN = dot(vOut, sp.geometricNormalInWorld);
         const float frontHit = primaryDotVN >= 0.0f ? 1.0f : -1.0f;
         const f3 positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
-        const ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+        ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+        if (BUMP) // :740-743
+            shadingFrame = bumpShadingFrameAtHit(s, mesh, gb0.z, bcB, bcC, shadingFrame);
         const BSDF bsdf = setupBsdfAtHit(s, mesh, gb0.z, bcB, bcC);
         createRadianceQuery(p, positionInWorld, shadingFrame.normal, vOut, bsdf, n.inferenceQuery + 14 * (size_t)pix);
     }
@@ -845,7 +865,10 @@ int launchNrcVisualizePrediction(gfx_ctx* ctx, cudaStream_t stream, const GfxFra
     const DevFrameParams p = makeDevParams(ctx, params);
     const dim3 block(8, 8), grid((F.W + 7) / 8, (F.H + 7) / 8);
     { GFX_TIMED(ctx, stream, "nrc_visualize_queries");
-    k_nrcVisualizeQueries<<<grid, block, 0, stream>>>(ctx->devScene(params), ctx->devFrame(), p, makeDevNrc(ctx)); }
+    if (params->enableBumpMapping)
+        k_nrcVisualizeQueries<true><<<grid, block, 0, stream>>>(ctx->devScene(params), ctx->devFrame(), p, makeDevNrc(ctx));
+    else
+        k_nrcVisualizeQueries<false><<<grid, block, 0, stream>>>(ctx->devScene(params), ctx->devFrame(), p, makeDevNrc(ctx)); }
     ctx->launches++;
     GFX_CUDA(ctx, cudaGetLastError());
     return GFX_OK;

@@ -60,8 +60,9 @@ GFX_D void shadeVertexVariant(const DevScene &s, const DevRegir &rg, const DevFr
     }
 }
 
-// pathTrace_rayGen_generic up to the path extension loop (:73-160)
-template <bool REGIR>
+// pathTrace_rayGen_generic up to the path extension loop (:73-160).  BUMP: GfxFrameParams::enableBumpMapping (a kernel of its own,
+// so that the frames without it run the code they ran before it existed; likewise k_ptBounce)
+template <bool REGIR, bool BUMP>
 __global__ void GFX_BOUNCE_BOUNDS k_ptFirstHit(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, DevRegir rg) {
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
     const uint32_t y = p.y0 + blockIdx.y * 8 + threadIdx.y;
@@ -90,7 +91,9 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptFirstHit(DevScene s, DevFrame f, DevFrameP
             const f3 vOut = normalize(p.camera.position - sp.positionInWorld);
             const float frontHit = dot(vOut, sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
             positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
-            const ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+            ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+            if (BUMP) // path_tracing :117-121, regir :200-203
+                shadingFrame = bumpShadingFrameAtHit(s, mesh, gb0.z, bcB, bcC, shadingFrame);
             const f3 vOutLocal = shadingFrame.toLocal(vOut);
 
             radiance = f3(0.0f);
@@ -112,7 +115,7 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptFirstHit(DevScene s, DevFrame f, DevFrameP
 
 // pathTrace_closestHit_generic (:218-300) + the bookkeeping of the path extension loop (:161-194) for the
 // compacted queue of live paths; `round` = pathLength - 2 selects the queue parity and the counters.
-template <bool REGIR>
+template <bool REGIR, bool BUMP>
 __global__ void GFX_BOUNCE_BOUNDS k_ptBounce(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, DevRegir rg, uint32_t round,
                                                  uint32_t maxLengthTerminate) {
     const uint32_t curQueue = round & 1u, nextQueue = curQueue ^ 1u;
@@ -156,7 +159,9 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptBounce(DevScene s, DevFrame f, DevFramePar
 
                 const f3 vOut = normalize(-rayDir);
                 const float frontHit = dot(vOut, sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
-                const ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+                ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+                if (BUMP) // path_tracing :252-255, regir :336-339
+                    shadingFrame = bumpShadingFrameAtHit(s, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), shadingFrame);
                 positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
                 const f3 vOutLocal = shadingFrame.toLocal(vOut);
 
@@ -449,6 +454,11 @@ static int launchPathTraceSvgf(gfx_ctx* ctx, cudaStream_t stream, const GfxFrame
 }
 
 int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int variant) {
+    if (params->enableBumpMapping && variant != GFX_PT_SVGF) {
+        const int rc = ensureBumpTable(ctx);
+        if (rc != GFX_OK)
+            return rc;
+    }
     if (variant == GFX_PT_NRC)
         return launchPathTraceNrc(ctx, stream, params);
     if (variant == GFX_PT_NRC_VISUALIZE_PREDICTION)
@@ -485,11 +495,16 @@ int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* par
 
     const dim3 block(8, 8);
     const dim3 grid((F.W + 7) / 8, (p.y1 - p.y0 + 7) / 8);
+    const bool bump = params->enableBumpMapping != 0;
     { GFX_TIMED(ctx, stream, "pt_first_hit");
-    if (regir)
-        k_ptFirstHit<true><<<grid, block, 0, stream>>>(s, f, p, ps, rg);
+    if (regir && bump)
+        k_ptFirstHit<true, true><<<grid, block, 0, stream>>>(s, f, p, ps, rg);
+    else if (regir)
+        k_ptFirstHit<true, false><<<grid, block, 0, stream>>>(s, f, p, ps, rg);
+    else if (bump)
+        k_ptFirstHit<false, true><<<grid, block, 0, stream>>>(s, f, p, ps, rg);
     else
-        k_ptFirstHit<false><<<grid, block, 0, stream>>>(s, f, p, ps, rg); }
+        k_ptFirstHit<false, false><<<grid, block, 0, stream>>>(s, f, p, ps, rg); }
     ctx->launches++;
     const int traceGrid = wavefrontGrid();
     int sms = 132;
@@ -502,10 +517,14 @@ int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* par
         { GFX_TIMED(ctx, stream, "pt_trace_extension"); k_traceWavefront<false, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.extRays[round & 1], c + 0, 0u, c + 1, extWriter); }
         const uint32_t maxLengthTerminate = (round + 2 >= maxPathLength || round + 1 == numRounds) ? 1u : 0u;
         GFX_TIMED(ctx, stream, "pt_bounce");
-        if (regir)
-            k_ptBounce<true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
+        if (regir && bump)
+            k_ptBounce<true, true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
+        else if (regir)
+            k_ptBounce<true, false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
+        else if (bump)
+            k_ptBounce<false, true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
         else
-            k_ptBounce<false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
+            k_ptBounce<false, false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
         ctx->launches += 3;
     }
     // the last round requests no rays (maxLengthTerminate), nothing is left in flight

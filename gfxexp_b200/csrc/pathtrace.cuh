@@ -96,6 +96,29 @@ GFX_D BSDF setupBsdfAtHit(const DevScene &s, const DevMesh &mesh, uint32_t primI
     return b;
 }
 
+// the bump of the shading frame at a hit of the path tracers (optix_pathtracing_kernels.cu:117-121, 252-255 and their copies in
+// regir and neural_radiance_caching): readModifiedNormal at computeSurfacePoint's texCoord (path_tracing_shared.h:509, 604),
+// interpolated here, out of line, only when the frame's enableBumpMapping is set
+static __device__ __noinline__ ReferenceFrame bumpShadingFrameAtHitOutOfLine(const uint4* bumpTable, const float4* bumpTexels,
+                                                                             const uint4* triangles, const float4* vertices,
+                                                                             uint32_t triBase, uint32_t vertexBase, uint32_t matSlot,
+                                                                             uint32_t primIndex, float bcB, float bcC,
+                                                                             ReferenceFrame frame) {
+    const uint4 tri = __ldg(triangles + triBase + primIndex);
+    const float4* vA = vertices + 3 * (size_t)(vertexBase + tri.x);
+    const float4* vB = vertices + 3 * (size_t)(vertexBase + tri.y);
+    const float4* vC = vertices + 3 * (size_t)(vertexBase + tri.z);
+    const float bcA = 1 - (bcB + bcC);
+    const f2 texCoord = bcA * f2(__ldg(vA).w, __ldg(vA + 1).w) + bcB * f2(__ldg(vB).w, __ldg(vB + 1).w) + bcC * f2(__ldg(vC).w, __ldg(vC + 1).w);
+    const uint4 b = __ldg(bumpTable + matSlot);
+    return applyBumpMapping(readModifiedNormal(bumpTexels + b.x, b.y, b.z, b.w, texCoord.x, texCoord.y), frame);
+}
+GFX_D ReferenceFrame bumpShadingFrameAtHit(const DevScene &s, const DevMesh &mesh, uint32_t primIndex, float bcB, float bcC,
+                                           const ReferenceFrame &frame) {
+    return bumpShadingFrameAtHitOutOfLine(s.bumpTable, s.bumpTexels, s.triangles, s.vertices, mesh.triBase, mesh.vertexBase,
+                                          mesh.materialSlot, primIndex, bcB, bcC, frame);
+}
+
 // path_tracing_shared.h:582-621 (first hit, from GBuffer0's quantised barycentrics)
 GFX_D void computeSurfacePointFromGBuffer(const DevScene &s, const DevInstance* inst, const DevMesh &mesh,
                                           uint32_t primIndex, float bcB, float bcC, SurfacePoint* sp) {

@@ -145,6 +145,11 @@ struct DevScene {
     const float4* texPool;
     const uint4* texTable;
     const uint4* materialTextures;
+    // bump maps: bumpTable[m] = (first texel in bumpTexels, width, height, GfxBumpMapType) of material m's map, or of the default
+    // 1x1 texel for a material without one (lights.cu uploadTextures, ensureBumpTable); only read by the BUMP variants of the
+    // kernels, which the host launches for frames with GfxFrameParams::enableBumpMapping
+    const uint4* bumpTable;
+    const float4* bumpTexels;
 };
 
 struct DevFrame {

@@ -11,6 +11,9 @@
 
 Materials (MaterialConvention::Traditional, :2219-2318): DiffuseAndSpecular with Kd / map_Kd, Ks / map_Ks, smoothness =
 sqrt(Ns) / 11 (:2271-2274), emittance = Ke (map_Ke is refused: textured emitters are not supported by the light sampler).
+Bump maps (:2280-2284, loadNormalTexture :1344-1356): `map_Bump` / `bump` (assimp's HEIGHT slot) before `norm` (NORMALS), UNORM
+texels without sRGB decode; a PNG with more than one channel is a normal map, a one-channel PNG (and spnza_bricks_a_bump.png) a
+height map -> Scene.bump_maps.
 Image textures are decoded the way the reference's samplers present them to the filter (sampler_sRGB: UNORM8 -> sRGB -> linear
 float, common_host.cpp:1462-1467) and handed over as fp32 RGBA (include/gfxb200.h GfxTextureDesc); PNG (8-bit, non-interlaced) is
 read here with zlib - the reference reads its images through stb_image / DDS loaders, which are file-format code outside the path.
@@ -29,6 +32,7 @@ from . import scenes
 
 F32 = np.float32
 NO_TEXTURE = 0xFFFFFFFF
+BUMP_NORMAL_MAP, BUMP_HEIGHT_MAP = 0, 1  # GfxBumpMapType
 
 
 # ---- PNG ---------------------------------------------------------------------------------------------------------------
@@ -145,6 +149,10 @@ def parse_mtl(path: str) -> Dict[str, dict]:
                 cur["Ns"] = float(tok[1])
             elif key in ("map_Kd", "map_Ks", "map_Ke"):
                 cur[key] = tok[-1]  # options (-s, -o ...) are not interpreted
+            elif key in ("map_Bump", "map_bump", "bump"):  # assimp's HEIGHT slot
+                cur["bump"] = tok[-1]  # options (-bm ...) are not interpreted either
+            elif key == "norm":  # assimp's NORMALS slot
+                cur["norm"] = tok[-1]
     return mats
 
 
@@ -200,10 +208,12 @@ def load_obj_scene(path: str, camera_position=(0.0, 1.0, 5.0), camera_orientatio
 
     materials = np.zeros(len(order), dtype=scenes.MATERIAL_DTYPE)
     material_textures = np.full((len(order), 4), NO_TEXTURE, dtype=np.uint32)
+    bump_maps = np.zeros((len(order), 2), dtype=np.uint32)
+    bump_maps[:, 0] = NO_TEXTURE
     textures: List[np.ndarray] = []
-    texture_index: Dict[Tuple[str, bool], int] = {}
+    texture_index: Dict[Tuple[str, bool], Tuple[int, int]] = {}
 
-    def texture(name: str, srgb: bool) -> int:
+    def texture_and_channels(name: str, srgb: bool) -> Tuple[int, int]:
         key = (name, srgb)
         if key not in texture_index:
             file = os.path.join(base, name)
@@ -212,9 +222,12 @@ def load_obj_scene(path: str, camera_position=(0.0, 1.0, 5.0), camera_orientatio
             else:
                 with open(file, "rb") as fh:
                     img = decode_png(fh.read())
-            texture_index[key] = len(textures)
+            texture_index[key] = (len(textures), 1 if img.ndim == 2 else img.shape[2])
             textures.append(image_to_texture(img, srgb))
         return texture_index[key]
+
+    def texture(name: str, srgb: bool) -> int:
+        return texture_and_channels(name, srgb)[0]
 
     meshes: List[scenes.Mesh] = []
     for mi, name in enumerate(order):
@@ -233,6 +246,13 @@ def load_obj_scene(path: str, camera_position=(0.0, 1.0, 5.0), camera_orientatio
             material_textures[mi, 0] = texture(m["map_Kd"], True)
         if "map_Ks" in m:
             material_textures[mi, 1] = texture(m["map_Ks"], True)
+        bump = m.get("bump", m.get("norm"))  # the HEIGHT slot first, then NORMALS (common_host.cpp:2280-2284)
+        if bump is not None:
+            # loadNormalTexture (common_host.cpp:1344-1356): UNORM texels (no sRGB decode); more than one channel = normal map,
+            # except the file the reference special-cases for Crytek Sponza
+            tex, channels = texture_and_channels(bump, False)
+            normal_map = channels > 1 and os.path.basename(bump) != "spnza_bricks_a_bump.png"
+            bump_maps[mi] = (tex, BUMP_NORMAL_MAP if normal_map else BUMP_HEIGHT_MAP)
 
         # aiProcess_JoinIdenticalVertices within the material group; GenNormals gives every face its own vertices
         tris = groups[name]
@@ -289,5 +309,8 @@ def load_obj_scene(path: str, camera_position=(0.0, 1.0, 5.0), camera_orientatio
                          math.radians(fov_y_deg), os.path.splitext(os.path.basename(path))[0])
     if textures:
         scene.textures = textures
-        scene.material_textures = material_textures
+        if (material_textures != NO_TEXTURE).any():  # otherwise every texture is a bump map
+            scene.material_textures = material_textures
+    if (bump_maps[:, 0] != NO_TEXTURE).any():
+        scene.bump_maps = bump_maps
     return scene

@@ -55,6 +55,7 @@ class Scene:
     env_map: Optional[np.ndarray] = None  # float32 [H, W, 4] equirectangular environment map (GfxSceneDesc::envTexels) or None
     textures: Optional[List[np.ndarray]] = None       # float32 [H, W, 4] images, linear (after sRGB decode)
     material_textures: Optional[np.ndarray] = None    # uint32 [numMaterials, 4]: texture of p0, p1, p2, emittance or 0xFFFFFFFF
+    bump_maps: Optional[np.ndarray] = None            # uint32 [numMaterials, 2]: bump-map texture or 0xFFFFFFFF, GfxBumpMapType
 
     @property
     def num_triangles(self) -> int:
@@ -519,6 +520,63 @@ def small_city_scene_textured() -> Scene:
     for mesh in scene.meshes:  # [0, 1] per face in the generator: stretch past the unit square, negative values included
         mesh.texcoords = (mesh.texcoords * F32(3.7) - F32(1.2)).astype(F32)
     scene.name = "small_city_textured"
+    return scene
+
+
+def unorm8(x: np.ndarray) -> np.ndarray:
+    """float32 texels as the texture unit reads a UNORM8 texture: round(255 x) / 255 (no sRGB decode)"""
+    return (np.round(np.clip(x, 0.0, 1.0) * 255.0).astype(F32) / F32(255.0)).astype(F32)
+
+
+def sine_normal_map(width: int, height: int, freq=(3, 2), amplitude: float = 0.6, seed: int = 21) -> np.ndarray:
+    """float32 [H, W, 4] normal map of the height field a sin(2 pi fx x / W) cos(2 pi fy y / H), stored as the reference reads
+    it: rgb = (n + 1) / 2 with y in the DirectX convention (readModifiedNormal flips it back), quantised to UNORM8.  One texel in
+    eight is shortened (x 0.6 .. 0.9) before quantisation, so that some decoded normals are far from unit length."""
+    rng = np.random.default_rng(seed)
+    y, x = np.mgrid[0:height, 0:width].astype(np.float64)
+    px, py = 2 * np.pi * freq[0] / width, 2 * np.pi * freq[1] / height
+    dhdx = amplitude * px * width / 8 * np.cos(px * x) * np.cos(py * y)
+    dhdy = -amplitude * py * height / 8 * np.sin(px * x) * np.sin(py * y)
+    n = np.stack([-dhdx, -dhdy, np.ones_like(x)], axis=-1)
+    n /= np.linalg.norm(n, axis=-1, keepdims=True)
+    n *= np.where(rng.random((height, width, 1)) < 0.125, rng.uniform(0.6, 0.9, (height, width, 1)), 1.0)
+    n[..., 1] = -n[..., 1]
+    out = np.ones((height, width, 4), dtype=F32)
+    out[..., :3] = unorm8((n + 1.0) * 0.5)
+    return out
+
+
+def noise_height_map(width: int, height: int, seed: int = 23) -> np.ndarray:
+    """float32 [H, W, 4] of a one-channel height map as stbi_load(..., 4) expands a grey PNG: (g, g, g, 1), g a smooth bump
+    pattern plus noise, quantised to UNORM8"""
+    rng = np.random.default_rng(seed)
+    y, x = np.mgrid[0:height, 0:width].astype(np.float64)
+    g = 0.5 + 0.3 * np.sin(2 * np.pi * 2 * x / width) * np.sin(2 * np.pi * 3 * y / height) + 0.15 * rng.random((height, width))
+    out = np.ones((height, width, 4), dtype=F32)
+    out[..., :3] = unorm8(g)[..., None]
+    return out
+
+
+def small_city_scene_bumped() -> Scene:
+    """small_city_scene_textured with bump maps (GfxSceneDesc::bumpMaps): a sinusoidal normal map with some texels of non-unit
+    length, a small non-square normal map, and one-channel height maps of non-power-of-two sizes, seeded.  Emitters and about a
+    quarter of the other materials have no map (the reference's default 1x1 texel)."""
+    scene = small_city_scene_textured()
+    base = len(scene.textures)
+    scene.textures = scene.textures + [sine_normal_map(48, 32), sine_normal_map(5, 3, (1, 1), 0.9, 29),
+                                       noise_height_map(37, 23), noise_height_map(6, 10, 31)]
+    maps = [(base, 0), (base + 1, 0), (base + 2, 1), (base + 3, 1)]  # (texture, GfxBumpMapType)
+    rng = np.random.default_rng(19)
+    n = scene.materials.shape[0]
+    bm = np.zeros((n, 2), dtype=np.uint32)
+    bm[:, 0] = 0xFFFFFFFF
+    for m in range(n):
+        pick = int(rng.integers(0, 5))
+        if scene.materials[m]["hasEmittance"] or pick == 4:
+            continue
+        bm[m] = maps[pick]
+    scene.bump_maps = bm
+    scene.name = "small_city_bumped"
     return scene
 
 

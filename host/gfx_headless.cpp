@@ -9,7 +9,9 @@
 //
 //   gfx_headless <scene.bin> <renderer> <width> <height> <frames> <out.raw> [nrc_params.f16] [-position-encoding tri|hash]
 //                [-view prediction|pathlength|flow|cells|noisy|variance|filtered-variance|albedo|normal|motion|samples]
-//                [-taa-jitter]
+//                [-taa-jitter] [-bump-mapping]
+//   -bump-mapping (every renderer but svgf): the apps' "Enable Bump Mapping" checkbox, GfxFrameParams::enableBumpMapping.  The
+//   scene file carries no textures, so every material reads the reference's default 1x1 bump texel.
 //   -position-encoding: the NRC network's position encoding, as the reference app's command line takes it
 //   (neural_radiance_caching_main.cpp:458, 755-766); hash grid by default.  nrc_params.f16 must hold that network's
 //   gfx_nrc_num_params halves.
@@ -116,7 +118,7 @@ int main(int argc, char** argv) {
     if (argc < 7) {
         fprintf(stderr, "usage: %s <scene.bin> <renderer> <width> <height> <frames> <out.raw | out.png> [nrc_params.f16] "
                 "[-position-encoding tri|hash] [-view prediction|pathlength|flow|cells|noisy|variance|filtered-variance|albedo|"
-                "normal|motion|samples] [-taa-jitter]\n", argv[0]);
+                "normal|motion|samples] [-taa-jitter] [-bump-mapping]\n", argv[0]);
         return 2;
     }
     const char* nrcParamsPath = nullptr;
@@ -124,6 +126,7 @@ int main(int argc, char** argv) {
     std::string view;
     int svgfView = -1; // GfxSVGFView of an SVGF app view
     bool taaJitter = false;
+    bool bumpMapping = false;
     for (int i = 7; i < argc; ++i) {
         const std::string arg = argv[i];
         if (arg == "-position-encoding" && i + 1 < argc) {
@@ -151,6 +154,8 @@ int main(int argc, char** argv) {
         }
         else if (arg == "-taa-jitter")
             taaJitter = true;
+        else if (arg == "-bump-mapping") // the apps' "Enable Bump Mapping" checkbox (perFramePlp.enableBumpMapping)
+            bumpMapping = true;
         else if (!nrcParamsPath && arg[0] != '-')
             nrcParamsPath = argv[i];
         else {
@@ -170,6 +175,10 @@ int main(int argc, char** argv) {
     }
     if (taaJitter && renderer != "svgf") {
         fprintf(stderr, "-taa-jitter needs the svgf renderer\n");
+        return 2;
+    }
+    if (bumpMapping && renderer == "svgf") { // the SVGF app has no bump mapping
+        fprintf(stderr, "-bump-mapping does not apply to the svgf renderer\n");
         return 2;
     }
     const uint32_t width = (uint32_t)atoi(argv[3]), height = (uint32_t)atoi(argv[4]);
@@ -207,6 +216,7 @@ int main(int argc, char** argv) {
         std::mt19937 perFrameRng(72139121);                                                // neural_radiance_caching_main.cpp:1602
 
         GfxFrameParams fp = scene.defaults;
+        fp.enableBumpMapping = bumpMapping ? 1u : 0u;
         uint32_t lastSpatialNeighborBaseIndex = 0, lastReservoirIndex = 1;                 // restir_di_main.cpp:1685-1686
         const uint32_t numSpatialReusePasses = 1;
         double totalMs = 0.0;

@@ -118,7 +118,23 @@ typedef struct GfxSceneDesc {
     const GfxTextureDesc* textures;
     const uint32_t* materialTextures;
     uint32_t numTextures;
+    /* bump maps (Material::texNormal + bumpMapType, common_host.cpp:1344-1412; MaterialData::normal + readModifiedNormal,
+     * common_device.cuh:205-240): bumpMaps[2 * m] = index into `textures` of material m's map, or 0xFFFFFFFF for the
+     * reference's default, the 1x1 texel (127, 127, 255) / 255 of createNormalTexture (createImmTexture quantises 0.5 to
+     * uint(255 * 0.5) = 127); bumpMaps[2 * m + 1] = its GfxBumpMapType (ignored, but must be valid, for 0xFFFFFFFF).  The maps
+     * are UNORM-decoded texels of the same pool as the other textures - no sRGB decode (sampler_normFloat) - sampled at level 0
+     * with repeat addressing.  gfx_scene_upload refuses an index past numTextures or an unknown type.  NULL = every material
+     * has the default texel.  Only read when GfxFrameParams::enableBumpMapping is set. */
+    const uint32_t* bumpMaps;
 } GfxSceneDesc;
+
+/* BumpMapTextureType (common_host.h): how a material's bump map is read (loadNormalTexture, common_host.cpp:1344-1356: a PNG
+ * with more than one channel is a normal map, a one-channel PNG - and spnza_bricks_a_bump.png - a height map) */
+typedef enum GfxBumpMapType {
+    GFX_BUMP_NORMAL_MAP = 0, /* readModifiedNormalFromNormalMap: n = 2 rgb - 1, n.y = -n.y (calcDimInfo's isLeftHanded = true) */
+    GFX_BUMP_HEIGHT_MAP = 1  /* readModifiedNormalFromHeightMap: tex2Dgather of channel 0, n = normalize(-dh/du, dh/dv, 1) with
+                              * dh/du = (5/1024 W) (g.y - g.x), dh/dv = (5/1024 H) (g.x - g.w) */
+} GfxBumpMapType;
 
 /* ---- BVH formats (bit-identical to the reference structs) ---------------------------- */
 
@@ -238,6 +254,15 @@ typedef struct GfxFrameParams {
     uint32_t enableEnvLight;
     float envLightPowerCoeff;
     float envLightRotation;
+    /* perFramePlp.enableBumpMapping, the "Enable Bump Mapping" checkbox (false by default: restir_di_main.cpp:1986, 2005, 2345;
+     * path_tracing_main.cpp:1516, 1537, 1765; regir_main.cpp:1728, 1755, 2011; neural_radiance_caching_main.cpp:1857, 1887,
+     * 2251).  When set, every shading frame built from a surface - gfx_gbuffer_launch (so also the ReSTIR passes, which read
+     * the frame back from the G-buffer) and the first hit and bounces of GFX_PT_BASELINE, GFX_PT_REGIR, GFX_PT_NRC and
+     * GFX_PT_NRC_VISUALIZE_PREDICTION - is tilted by applyBumpMapping(readModifiedNormal(GfxSceneDesc::bumpMaps of the
+     * material, texCoord)) before anything reads it.  As in the reference, a material without a map is tilted too, by about
+     * 0.3 degrees (the default texel decodes to (-1/255, 1/255, 1)).  The SVGF app has no such switch: GFX_PT_SVGF ignores
+     * the flag, and since gfx_gbuffer_launch (with or without GFX_SVGF_SUBPIXEL_JITTER) does not, an SVGF host leaves it 0. */
+    uint32_t enableBumpMapping;
 } GfxFrameParams;
 
 typedef enum GfxSVGFFlags {
@@ -505,6 +530,14 @@ int gfx_light_pick_debug(gfx_ctx* ctx, void* stream, const float* ul, uint32_t n
  * op 0: RegularConstantContinuousDistribution2D::sample(u0, u1) -> (u, v, uvPDF); 1: evaluatePDF(u, v) -> (pdf, 0, 0);
  * 2: the software tex2DLod of the map at (u, v) -> rgb */
 int gfx_env_light_debug(gfx_ctx* ctx, void* stream, int op, const float* in, uint32_t n, float* out);
+/* test hook of the bump mapping (GfxSceneDesc::bumpMaps), n DEVICE records in and out:
+ * op 0: readModifiedNormal of material matSlot's map at (u, v): 2 floats in, 3 out;
+ * op 1: applyBumpMapping(modified normal, frame): 12 floats in (modified normal, tangent, bitangent, normal), 9 out (the frame);
+ * op 2: the four channel-0 texels of the 2x2 footprint at (u, v) of material matSlot's map in tex2Dgather's order: 2 floats in,
+ *       8 out = the software gather of the kernels, then the texture unit's tld4 on a CUDA texture object made from the same map
+ *       (a uchar4 cudaArray holding round(255 texel), normalised-float read, repeat addressing, linear filter).
+ * GFX_ERR_NOT_READY before gfx_scene_upload, GFX_ERR_INVALID_ARGUMENT for another op or a material slot out of range. */
+int gfx_bump_debug(gfx_ctx* ctx, void* stream, int op, uint32_t matSlot, const float* in, uint32_t n, float* out);
 /* host read-back of the instance-level distribution for parity: weights/cdf sized numInstances */
 int gfx_light_dist_export(gfx_ctx* ctx, float* instWeights, float* instCdf, float* integral);
 
@@ -545,7 +578,7 @@ int gfx_svgf_launch(gfx_ctx* ctx, void* stream, const GfxFrameParams* params, in
  *   ALBEDO             the SVGF albedo (the thresholded DH reflectance of the temporal pass; 1 at background pixels)
  *   NORMAL             0.5 n + 0.5 of the shading normal the temporal pass decoded.  The app reads its G-buffer, which it never
  *                      clears (svgf_main.cpp:2036-2042), so its background pixels show stale normals; here n = 0 there, and they
- *                      show (0.5, 0.5, 0.5).  The normal is not bump-mapped: the library has no bump mapping.
+ *                      show (0.5, 0.5, 0.5).  The normal is not bump-mapped: the SVGF app has no bump mapping.
  *   MOTION_VECTOR      mv = (W, H) * ((x + 0.5, y + 0.5) / (W, H) - prevScreenPos), the prevScreenPos of the temporal pass (hits)
  *                      and of GFX_SVGF_FILL_BACKGROUND (background); clamp(scale * mv + offset, 0, 1) in r and g, b = offset
  *   SAMPLE_COUNT       min(count / 255, 1), count = the low 24 bits of GFX_BUF_SVGF_MOMENTS[params->bufferIndex].z
