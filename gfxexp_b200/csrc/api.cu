@@ -733,6 +733,13 @@ int gfx_env_light_debug(gfx_ctx* ctx, void* stream, int op, const float* in, uin
     return debugEnvLight(ctx, (cudaStream_t)stream, op, in, n, out);
 }
 
+int gfx_shading_debug(gfx_ctx* ctx, void* stream, int op, const float* material, const float* in, uint32_t n, float* out) {
+    CHECK_CTX(ctx);
+    if (!material || (n && (!in || !out)) || op < 0 || op > 15)
+        return GFX_ERR_INVALID_ARGUMENT;
+    return debugShading(ctx, (cudaStream_t)stream, op, material, in, n, out);
+}
+
 int gfx_bump_debug(gfx_ctx* ctx, void* stream, int op, uint32_t matSlot, const float* in, uint32_t n, float* out) {
     CHECK_CTX(ctx);
     if (!ctx->scene.uploaded)

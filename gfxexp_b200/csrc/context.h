@@ -278,6 +278,7 @@ int buildLightDistributions(gfx_ctx* ctx, cudaStream_t stream, uint32_t bufferIn
 int uploadEnvLight(gfx_ctx* ctx, const float* rgba, uint32_t width, uint32_t height);
 int uploadTextures(gfx_ctx* ctx, const GfxSceneDesc* sd);
 int debugEnvLight(gfx_ctx* ctx, cudaStream_t stream, int op, const float* dIn, uint32_t n, float* dOut);
+int debugShading(gfx_ctx* ctx, cudaStream_t stream, int op, const float* material, const float* dIn, uint32_t n, float* dOut);
 int ensureBumpTable(gfx_ctx* ctx); // lights.cu, before a launch with enableBumpMapping
 int debugBump(gfx_ctx* ctx, cudaStream_t stream, int op, uint32_t matSlot, const float* dIn, uint32_t n, float* dOut);
 int debugLightPick(gfx_ctx* ctx, cudaStream_t stream, const float* dUl, uint32_t n, uint32_t* dFlat, uint32_t* dChain);

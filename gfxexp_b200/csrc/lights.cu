@@ -20,6 +20,7 @@
 //    material emittance, i.e. the operands sampleLight (restir_di_shared.h:417-425,485-511) would
 //    recompute for each of the 66 M candidates per frame.
 #include "lighting.cuh"
+#include "shading_debug.cuh"
 #include "context.h"
 #include <cmath>
 #include <algorithm>
@@ -667,6 +668,33 @@ int debugEnvLight(gfx_ctx* ctx, cudaStream_t stream, int op, const float* dIn, u
     }
     if (n)
         k_envDebug<<<(n + 127) / 128, 128, 0, stream>>>(s.env, op, reinterpret_cast<const float2*>(dIn), n, dOut);
+    ctx->launches++;
+    GFX_CUDA(ctx, cudaGetLastError());
+    return GFX_OK;
+}
+
+// test hook (gfx_shading_debug): one op of the shading layer's table (shading_debug.cuh) per record; needs no scene
+static_assert(kShadingDebugNumOps == 16, "gfx_shading_debug accepts ops 0..15");
+struct ShadingDebugMaterial {
+    float m[9];
+};
+__global__ void k_shadingDebug(int op, ShadingDebugMaterial mat, const float* in, uint32_t n, float* out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    float a[kShadingDebugStride], o[kShadingDebugStride];
+    for (int k = 0; k < kShadingDebugStride; ++k)
+        a[k] = in[kShadingDebugStride * (size_t)i + k];
+    shadingDebugOp(op, mat.m, a, o);
+    for (int k = 0; k < kShadingDebugStride; ++k)
+        out[kShadingDebugStride * (size_t)i + k] = o[k];
+}
+int debugShading(gfx_ctx* ctx, cudaStream_t stream, int op, const float* material, const float* dIn, uint32_t n, float* dOut) {
+    ShadingDebugMaterial mat;
+    for (int k = 0; k < 9; ++k)
+        mat.m[k] = material[k];
+    if (n)
+        k_shadingDebug<<<(n + 127) / 128, 128, 0, stream>>>(op, mat, dIn, n, dOut);
     ctx->launches++;
     GFX_CUDA(ctx, cudaGetLastError());
     return GFX_OK;

@@ -530,6 +530,16 @@ int gfx_light_pick_debug(gfx_ctx* ctx, void* stream, const float* ul, uint32_t n
  * op 0: RegularConstantContinuousDistribution2D::sample(u0, u1) -> (u, v, uvPDF); 1: evaluatePDF(u, v) -> (pdf, 0, 0);
  * 2: the software tex2DLod of the map at (u, v) -> rgb */
 int gfx_env_light_debug(gfx_ctx* ctx, void* stream, int op, const float* in, uint32_t n, float* out);
+/* test hook of the shading layer every renderer shares (BSDFs, sampling warps, encoders, frames); needs no scene.
+ * material: 9 HOST floats {bsdfType, p0[3], p1[3], p2, regularize != 0}, read as setupBSDFBody reads a material with 1x1
+ * textures (regularize = BSDFFlags::Regularize).  in / out: n DEVICE records of 8 floats each, unused output slots 0, integer
+ * codes as their bits.  op 0: evaluate(vGiven, vSampled) -> rgb; 1: evaluatePDF(vGiven, vSampled); 2: sampleThroughput(vGiven,
+ * u0, u1) -> (rgb, vSampled, dirPDensity); 3: evaluateDHReflectanceEstimate(vGiven) -> rgb; 4: concentricSampleDisk(u0, u1);
+ * 5: cosineSampleHemisphere(u0, u1); 6: toPolarYUp(v) -> (phi, theta); 7: fromPolarYUp(phi, theta); 8: encodeVector(v);
+ * 9: decodeVector(code); 10: encodeBarycentric(bc); 11: decodeBarycentric(code); 12: encodeTexCoords(u, v);
+ * 13: decodeTexCoords(code); 14: makeCoordinateSystem(normal) -> (tangent, bitangent); 15: offsetRayOrigin(p, n).
+ * GFX_ERR_INVALID_ARGUMENT for another op or a missing pointer. */
+int gfx_shading_debug(gfx_ctx* ctx, void* stream, int op, const float* material, const float* in, uint32_t n, float* out);
 /* test hook of the bump mapping (GfxSceneDesc::bumpMaps), n DEVICE records in and out:
  * op 0: readModifiedNormal of material matSlot's map at (u, v): 2 floats in, 3 out;
  * op 1: applyBumpMapping(modified normal, frame): 12 floats in (modified normal, tangent, bitangent, normal), 9 out (the frame);

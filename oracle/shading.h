@@ -182,7 +182,10 @@ struct BSDF {
     float3 specularF0Color;
     float roughness;
 
-    // setupBSDFBody<...> (common_device.cuh:376-385, 778-826) with 1x1 textures
+    // setupBSDFBody<...> (common_device.cuh:376-385, 778-826) with 1x1 textures.  REGULARIZE = BSDFFlags::Regularize
+    // (:795-797, :821-823): the smoothness is halved, for DiffuseAndSpecular before the 0.999 clamp, for SimplePBR after it;
+    // Lambert ignores the flag.
+    template <bool REGULARIZE = false>
     void setup(uint32_t bsdfType, const float* p0, const float* p1, float p2) {
         if (bsdfType == 0) {
             type = 0;
@@ -192,7 +195,10 @@ struct BSDF {
         }
         else if (bsdfType == 1) {
             type = 1;
-            const float smoothness = std::fmin(p2, 0.999f);
+            float smoothness = p2;
+            if (REGULARIZE)
+                smoothness *= 0.5f;
+            smoothness = std::fmin(smoothness, 0.999f);
             diffuseColor = float3(p0[0], p0[1], p0[2]);
             specularF0Color = float3(p1[0], p1[1], p1[2]);
             roughness = 1 - smoothness;
@@ -200,7 +206,9 @@ struct BSDF {
         else { // SimplePBR_BRDF(baseColor, 0.5f, smoothness, metallic) :767-776, :806-826
             type = 1;
             const float3 baseColor(p0[0], p0[1], p0[2]);
-            const float smoothness = std::fmin(1.0f - p1[1], 0.999f);
+            float smoothness = std::fmin(1.0f - p1[1], 0.999f);
+            if (REGULARIZE)
+                smoothness *= 0.5f;
             const float metallic = p1[2];
             const float reflectance = 0.5f;
             diffuseColor = baseColor * (1 - metallic);

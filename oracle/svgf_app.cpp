@@ -43,28 +43,7 @@ BSDF setupBsdfRegularized(const orc_scene* s, uint32_t matSlot, const float2 &te
         }
     }
     BSDF b;
-    if (m.bsdfType == 0) {
-        b.setup(m.bsdfType, p0, p1, p2);
-    }
-    else if (m.bsdfType == 1) {
-        float smoothness = p2;
-        smoothness *= 0.5f;
-        b.type = 1;
-        b.diffuseColor = float3(p0[0], p0[1], p0[2]);
-        b.specularF0Color = float3(p1[0], p1[1], p1[2]);
-        b.roughness = 1 - std::fmin(smoothness, 0.999f);
-    }
-    else {
-        const float3 baseColor(p0[0], p0[1], p0[2]);
-        float smoothness = std::fmin(1.0f - p1[1], 0.999f);
-        const float metallic = p1[2];
-        smoothness *= 0.5f;
-        const float reflectance = 0.5f;
-        b.type = 1;
-        b.diffuseColor = baseColor * (1 - metallic);
-        b.specularF0Color = float3(0.16f * pow2(reflectance) * (1 - metallic)) + baseColor * metallic;
-        b.roughness = 1 - smoothness;
-    }
+    b.setup<true>(m.bsdfType, p0, p1, p2);
     return b;
 }
 
