@@ -396,6 +396,7 @@ _DECLS = {
     "gfx_launch_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(GfxBatchOp), c_u32]),
     "gfx_light_pick_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, c_u32, C.c_void_p, C.c_void_p]),
     "gfx_env_light_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, c_u32, C.c_void_p]),
+    "gfx_light_sample_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, c_u32, C.c_void_p]),
     "gfx_shading_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, c_u32, C.c_void_p]),
     "gfx_bump_debug": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, c_u32, C.c_void_p, c_u32, C.c_void_p]),
     "gfx_light_dist_export": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(c_f)]),

@@ -202,7 +202,9 @@ DevScene gfx_ctx::devScene() const {
 }
 DevScene gfx_ctx::devScene(const GfxFrameParams* p) const {
     DevScene d = devScene();
-    d.env.enabled = scene.envW != 0 && p->enableEnvLight ? 1u : 0u; // plp.s->envLightTexture && plp.f->enableEnvLight
+    // plp.s->envLightTexture && plp.f->enableEnvLight; a map that is black everywhere has nothing to sample (its importance map has
+    // integral 0, so every density would be 0) and is treated as no environment light (DESIGN.md, "Environment maps with black rows")
+    d.env.enabled = scene.envW != 0 && scene.envIntegral > 0.0f && p->enableEnvLight ? 1u : 0u;
     d.env.powerCoeff = p->envLightPowerCoeff;
     d.env.rotation = p->envLightRotation;
     return d;
@@ -731,6 +733,15 @@ int gfx_env_light_debug(gfx_ctx* ctx, void* stream, int op, const float* in, uin
     if ((n && (!in || !out)) || op < 0 || op > 2)
         return GFX_ERR_INVALID_ARGUMENT;
     return debugEnvLight(ctx, (cudaStream_t)stream, op, in, n, out);
+}
+
+int gfx_light_sample_debug(gfx_ctx* ctx, void* stream, int op, const float* params, const float* in, uint32_t n, float* out) {
+    CHECK_CTX(ctx);
+    if (!ctx->scene.uploaded || ctx->scene.pickDirty || ctx->scene.lightTrisDirty)
+        return GFX_ERR_NOT_READY;
+    if (!params || (n && (!in || !out)) || op < 0 || op > 7)
+        return GFX_ERR_INVALID_ARGUMENT;
+    return debugLightSample(ctx, (cudaStream_t)stream, op, params, in, n, out);
 }
 
 int gfx_shading_debug(gfx_ctx* ctx, void* stream, int op, const float* material, const float* in, uint32_t n, float* out) {

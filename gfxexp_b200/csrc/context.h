@@ -55,6 +55,7 @@ struct SceneState {
     float* envTopPdf = nullptr;
     float* envTopCdf = nullptr;
     uint32_t envW = 0, envH = 0;
+    float envIntegral = 0.0f;              // integral of the importance map; 0 for a black map, which is no light to sample
     uint2* pickPieces = nullptr;           // pickCapacity + 2
     uint32_t* pickKeyAt = nullptr;         // kPickGuideSize + 1
     uint4* pickQueue[2] = { nullptr, nullptr };
@@ -282,6 +283,7 @@ int debugShading(gfx_ctx* ctx, cudaStream_t stream, int op, const float* materia
 int ensureBumpTable(gfx_ctx* ctx); // lights.cu, before a launch with enableBumpMapping
 int debugBump(gfx_ctx* ctx, cudaStream_t stream, int op, uint32_t matSlot, const float* dIn, uint32_t n, float* dOut);
 int debugLightPick(gfx_ctx* ctx, cudaStream_t stream, const float* dUl, uint32_t n, uint32_t* dFlat, uint32_t* dChain);
+int debugLightSample(gfx_ctx* ctx, cudaStream_t stream, int op, const float* params, const float* dIn, uint32_t n, float* dOut);
 size_t lightPickSortTempBytes(uint32_t capacity);
 int launchGBuffer(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p);
 int launchReSTIR(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int pass);

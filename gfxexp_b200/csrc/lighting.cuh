@@ -351,21 +351,33 @@ GFX_D bool chooseEnvForNee(const DevScene &s, float* uLight, float* probToSample
     return false;
 }
 // the miss programs of the path tracers (optix_pathtracing_kernels.cu:310-341; neural_radiance_caching/...:625-650, which
-// multiplies by probToSampleEnvLight unconditionally): luminance x MIS weight of the environment along rayDir
-static __device__ __noinline__ f3 evaluateEnvLightOnMissOutOfLine(DevEnvLight env, f3 rayDirIn, float prevDirPDensity, float probToSampleEnv) {
+// multiplies by probToSampleEnvLight unconditionally), in three parts that gfx_light_sample_debug op 4 shares: the texture
+// coordinates of rayDir, the density with which sampleEnvLight would have produced it, and the MIS weight of the environment
+GFX_D void envMissCoordinates(const DevEnvLight &env, const f3 &rayDirIn, float* tu, float* tv, float* theta) {
     const f3 rayDir = normalize(rayDirIn);
-    float posPhi, theta;
-    toPolarYUp(rayDir, &posPhi, &theta);
+    float posPhi;
+    toPolarYUp(rayDir, &posPhi, theta);
     float phi = posPhi + env.rotation;
     phi = phi - floorf(phi / (2 * kPi)) * 2 * kPi;
-    const float tu = phi / (2 * kPi), tv = theta / kPi;
-    const f3 luminance = env.powerCoeff * envFetchOutOfLine(env, tu, tv);
+    *tu = phi / (2 * kPi);
+    *tv = *theta / kPi;
+}
+GFX_D float envMissHypAreaPDensity(const DevEnvLight &env, float tu, float tv, float theta) {
     const float uvPDF = envEvaluatePDF(env, tu, tv);
-    const float hypAreaPDensity = uvPDF / (2 * kPi * kPi * dm_sin(theta));
+    return uvPDF / (2 * kPi * kPi * dm_sin(theta));
+}
+GFX_D float envMissMisWeight(float hypAreaPDensity, float prevDirPDensity, float probToSampleEnv) {
     const float lightPDensity = probToSampleEnv * hypAreaPDensity;
     const float bsdfPDensity = prevDirPDensity;
-    const float misWeight = pow2f(bsdfPDensity) / (pow2f(bsdfPDensity) + pow2f(lightPDensity));
-    return luminance * misWeight;
+    return pow2f(bsdfPDensity) / (pow2f(bsdfPDensity) + pow2f(lightPDensity));
+}
+// luminance x MIS weight of the environment along rayDir
+static __device__ __noinline__ f3 evaluateEnvLightOnMissOutOfLine(DevEnvLight env, f3 rayDirIn, float prevDirPDensity, float probToSampleEnv) {
+    float tu, tv, theta;
+    envMissCoordinates(env, rayDirIn, &tu, &tv, &theta);
+    const f3 luminance = env.powerCoeff * envFetchOutOfLine(env, tu, tv);
+    const float hypAreaPDensity = envMissHypAreaPDensity(env, tu, tv, theta);
+    return luminance * envMissMisWeight(hypAreaPDensity, prevDirPDensity, probToSampleEnv);
 }
 GFX_D f3 evaluateEnvLightOnMiss(const DevScene &s, const f3 &rayDir, float prevDirPDensity, bool nrcVariant) {
     const float probToSampleEnv = (nrcVariant || __ldg(s.instIntegral) > 0.0f) ? kProbToSampleEnvLight : 1.0f;

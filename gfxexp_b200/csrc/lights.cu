@@ -19,7 +19,7 @@
 //    (inst.transform * v.position), recArea = 2 / |cross|, the object-space vertex normals and the
 //    material emittance, i.e. the operands sampleLight (restir_di_shared.h:417-425,485-511) would
 //    recompute for each of the 66 M candidates per frame.
-#include "lighting.cuh"
+#include "pathtrace.cuh"
 #include "shading_debug.cuh"
 #include "context.h"
 #include <cmath>
@@ -515,6 +515,9 @@ struct KahanSum { // CompensatedSum_T<float>, basic_types.h:5427-5452
         result = sumTemp;
     }
 };
+// Integral 0 (a black row, or a black map): the reference's lines divide 0 by 0 and leave NaN in every pdf and CDF entry, which
+// reaches the miss programs' MIS weights; here such a distribution gets pdf 0 and the uniform CDF i / n instead (DESIGN.md,
+// "Environment maps with black rows").  Every other distribution is the reference's, bit for bit.
 float regularDistribution(const float* values, uint32_t n, float* pdf, float* cdf) {
     KahanSum sum;
     for (uint32_t i = 0; i < n; ++i) {
@@ -523,8 +526,14 @@ float regularDistribution(const float* values, uint32_t n, float* pdf, float* cd
     }
     const float integral = sum.result;
     for (uint32_t i = 0; i < n; ++i) {
-        pdf[i] = values[i] / integral;
-        cdf[i] /= integral;
+        if (integral > 0.0f) {
+            pdf[i] = values[i] / integral;
+            cdf[i] /= integral;
+        }
+        else {
+            pdf[i] = 0.0f;
+            cdf[i] = (float)i / (float)n;
+        }
     }
     cdf[n] = 1.0f;
     return integral;
@@ -543,6 +552,10 @@ int uploadEnvLight(gfx_ctx* ctx, const float* rgba, uint32_t width, uint32_t hei
         const float sinTheta = std::sin(theta);
         for (uint32_t x = 0; x < width; ++x) {
             const float* src = rgba + 4 * ((size_t)y * width + x);
+            if (std::isnan(src[0]) || std::isnan(src[1]) || std::isnan(src[2])) { // the clamp below would pass it into every pdf
+                ctx->setError("gfx_scene_upload: NaN texel in the environment map");
+                return GFX_ERR_INVALID_ARGUMENT;
+            }
             float4 t;
             t.x = std::min(std::max(src[0], 0.0f), 65504.0f);
             t.y = std::min(std::max(src[1], 0.0f), 65504.0f);
@@ -555,7 +568,7 @@ int uploadEnvLight(gfx_ctx* ctx, const float* rgba, uint32_t width, uint32_t hei
     for (uint32_t y = 0; y < height; ++y)
         rowIntegral[y] = regularDistribution(importance.data() + (size_t)y * width, width, pdf.data() + (size_t)y * width,
                                              cdf.data() + (size_t)y * (width + 1));
-    regularDistribution(rowIntegral.data(), height, topPdf.data(), topCdf.data());
+    const float integral = regularDistribution(rowIntegral.data(), height, topPdf.data(), topCdf.data());
     auto upload = [&](void** dst, const void* src, size_t bytes) {
         cudaError_t e = cudaMalloc(dst, bytes);
         if (e == cudaSuccess)
@@ -569,6 +582,7 @@ int uploadEnvLight(gfx_ctx* ctx, const float* rgba, uint32_t width, uint32_t hei
     GFX_CUDA(ctx, upload((void**)&S.envTopCdf, topCdf.data(), topCdf.size() * 4));
     S.envW = width;
     S.envH = height;
+    S.envIntegral = integral;
     return GFX_OK;
 }
 
@@ -668,6 +682,97 @@ int debugEnvLight(gfx_ctx* ctx, cudaStream_t stream, int op, const float* dIn, u
     }
     if (n)
         k_envDebug<<<(n + 127) / 128, 128, 0, stream>>>(s.env, op, reinterpret_cast<const float2*>(dIn), n, dOut);
+    ctx->launches++;
+    GFX_CUDA(ctx, cudaGetLastError());
+    return GFX_OK;
+}
+
+// test hook (gfx_light_sample_debug): light sampling as the renderers call it, one record of kLightSampleDebugStride floats in and
+// out per op (include/gfxb200.h lists the layouts); integers travel as their bits
+constexpr int kLightSampleDebugStride = 16;
+__global__ void k_lightSampleDebug(DevScene s, int op, const float* __restrict__ in, uint32_t n, float* __restrict__ out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n)
+        return;
+    const float* a = in + kLightSampleDebugStride * (size_t)i;
+    float o[kLightSampleDebugStride];
+    for (int k = 0; k < kLightSampleDebugStride; ++k)
+        o[k] = 0.0f;
+    if (op <= 2) {
+        const float ul = a[0], u0 = a[1], u1 = a[2];
+        const f3 shadingPoint(a[3], a[4], a[5]), shadingNormal(a[6], a[7], a[8]);
+        const float vOutLocalZ = a[9];
+        LightSample ls = emptyLightSample();
+        float density = 0.0f, lightProb = 0.0f;
+        bool dark = false;
+        if (op == 0) {
+            sampleLight(s, ul, u0, u1, &ls, &density);
+        }
+        else if (op == 1) {
+            dark = sampleLightUnlessDark(s, ul, u0, u1, shadingPoint, shadingNormal, vOutLocalZ, &ls, &density);
+        }
+        else {
+            const uint32_t code = classifyLight(s, ul, pickGuideFetch(s, ul), shadingPoint, shadingNormal, vOutLocalZ);
+            dark = code == kLightDark || finishLightSample(s, code, u0, u1, shadingPoint, shadingNormal, vOutLocalZ, &ls, &density);
+        }
+        o[0] = __uint_as_float(pickLightTriangle(s, ul));
+        chainPickLightTriangle(s, ul, &lightProb);
+        o[1] = ls.position.x; o[2] = ls.position.y; o[3] = ls.position.z;
+        o[4] = ls.normal.x; o[5] = ls.normal.y; o[6] = ls.normal.z;
+        o[7] = ls.emittance.x; o[8] = ls.emittance.y; o[9] = ls.emittance.z;
+        o[10] = density;
+        o[11] = lightProb;
+        o[12] = dark ? 1.0f : 0.0f;
+    }
+    else if (op == 3) {
+        LightSample ls = emptyLightSample();
+        float density = 0.0f;
+        sampleEnvLight(s, a[0], a[1], &ls, &density);
+        o[0] = ls.position.x; o[1] = ls.position.y; o[2] = ls.position.z;
+        o[3] = density;
+        o[4] = ls.emittance.x; o[5] = ls.emittance.y; o[6] = ls.emittance.z;
+    }
+    else if (op == 4) {
+        float tu, tv, theta;
+        envMissCoordinates(s.env, f3(a[0], a[1], a[2]), &tu, &tv, &theta);
+        o[0] = envMissHypAreaPDensity(s.env, tu, tv, theta);
+        o[1] = envMissMisWeight(o[0], a[3], a[4]);
+        o[2] = tu; o[3] = tv;
+    }
+    else if (op == 5) {
+        const uint32_t instSlot = __float_as_uint(a[0]), geomInInst = __float_as_uint(a[1]), primIndex = __float_as_uint(a[2]);
+        if (instSlot < s.numInstances && geomInInst < s.instances[instSlot].numMeshSlots) {
+            const DevInstance* inst = s.instances + instSlot;
+            const DevMesh mesh = s.meshes[s.instanceMeshSlots[inst->firstMeshSlot + geomInInst]];
+            if (primIndex < mesh.numTriangles) {
+                SurfacePoint sp;
+                computeSurfacePointAtHit(s, inst, mesh, primIndex, a[3], a[4], &sp);
+                o[0] = sp.hypAreaPDensity;
+            }
+        }
+    }
+    else {
+        float ul = op == 6 ? a[2] : a[0], prob = 0.0f;
+        const bool env = op == 6 ? chooseEnvForCandidate(s, __float_as_uint(a[0]), __float_as_uint(a[1]), &ul, &prob)
+                                 : chooseEnvForNee(s, &ul, &prob);
+        o[0] = env ? 1.0f : 0.0f; o[1] = ul; o[2] = prob;
+    }
+    for (int k = 0; k < kLightSampleDebugStride; ++k)
+        out[kLightSampleDebugStride * (size_t)i + k] = o[k];
+}
+int debugLightSample(gfx_ctx* ctx, cudaStream_t stream, int op, const float* params, const float* dIn, uint32_t n, float* dOut) {
+    GfxFrameParams p;
+    memset(&p, 0, sizeof(p));
+    p.envLightRotation = params[0];
+    p.envLightPowerCoeff = params[1];
+    p.enableEnvLight = params[2] != 0.0f ? 1u : 0u;
+    const DevScene s = ctx->devScene(&p);
+    if ((op == 3 || op == 4) && !s.env.W) {
+        ctx->setError("gfx_light_sample_debug: the scene has no environment map");
+        return GFX_ERR_NOT_READY;
+    }
+    if (n)
+        k_lightSampleDebug<<<(n + 127) / 128, 128, 0, stream>>>(s, op, dIn, n, dOut);
     ctx->launches++;
     GFX_CUDA(ctx, cudaGetLastError());
     return GFX_OK;

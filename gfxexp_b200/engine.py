@@ -112,6 +112,20 @@ class Context:
     def build_light_distributions(self, buffer_index: int = 0, stream=None):
         self._check(self.lib.gfx_light_dist_build(self.h, stream, buffer_index), "gfx_light_dist_build")
 
+    def light_sample_debug(self, op: int, records: np.ndarray, env_rotation: float = 0.0, env_power: float = 1.0,
+                           enable_env: bool = False) -> np.ndarray:
+        """gfx_light_sample_debug: records [n, <= 16] float32 (integers as their bits) -> [n, 16] float32"""
+        import torch
+        a = np.zeros((records.shape[0], 16), dtype=np.float32)
+        a[:, :records.shape[1]] = records
+        d_in = torch.from_numpy(a).cuda()
+        d_out = torch.empty_like(d_in)
+        params = (C.c_float * 3)(env_rotation, env_power, 1.0 if enable_env else 0.0)
+        self._check(self.lib.gfx_light_sample_debug(self.h, None, op, params, d_in.data_ptr(), a.shape[0], d_out.data_ptr()),
+                    "gfx_light_sample_debug")
+        torch.cuda.synchronize()
+        return d_out.cpu().numpy()
+
     def light_dist(self):
         n = len(self._scene_arrays.scene.instances)
         w = np.zeros(n, dtype=np.float32)

@@ -530,6 +530,24 @@ int gfx_light_pick_debug(gfx_ctx* ctx, void* stream, const float* ul, uint32_t n
  * op 0: RegularConstantContinuousDistribution2D::sample(u0, u1) -> (u, v, uvPDF); 1: evaluatePDF(u, v) -> (pdf, 0, 0);
  * 2: the software tex2DLod of the map at (u, v) -> rgb */
 int gfx_env_light_debug(gfx_ctx* ctx, void* stream, int op, const float* in, uint32_t n, float* out);
+/* test hook of light sampling as the renderers call it (lighting.cuh, pathtrace.cuh).  params: 3 HOST floats {envLightRotation,
+ * envLightPowerCoeff, enableEnvLight != 0}, read as a frame's GfxFrameParams.  in / out: n DEVICE records of 16 floats each, unused
+ * output slots 0, integers as their bits.
+ * op 0: sampleLight(ul, u0, u1): in (ul, u0, u1); out (key of the flattened pick, position, normal, emittance, areaPDensity, the
+ *       chain's lightProb (0 for a probability-0 early out), 0);
+ * op 1: sampleLightUnlessDark(ul, u0, u1, shadingPoint, shadingNormal, vOutLocalZ): in (ul, u0, u1, point.xyz, normal.xyz,
+ *       vOutLocalZ); out as op 0 with slot 12 = 1 for "dark";
+ * op 2: classifyLight + finishLightSample (the two-phase candidate loop, guide entry from pickGuideFetch) on op 1's inputs and outputs;
+ * op 3: sampleEnvLight(u0, u1): in (u0, u1); out (direction, areaPDensity, emittance);
+ * op 4: the miss programs' density of the environment along a direction: in (direction, prevDirPDensity, probToSampleEnv); out
+ *       (hypAreaPDensity, misWeight, u, v);
+ * op 5: computeSurfacePointAtHit's hypAreaPDensity: in (instance slot, geometry index in the instance, primitive, bcB, bcC); out
+ *       (hypAreaPDensity), 0 for indices out of range;
+ * op 6: chooseEnvForCandidate(i, n, ul): in (i, n, ul); op 7: chooseEnvForNee(ul): in (ul); out (environment chosen, remapped ul,
+ *       probToSampleCurLightType).
+ * GFX_ERR_NOT_READY before gfx_scene_upload, before gfx_light_dist_build has built the light pick of the current transforms, and for
+ * ops 3 and 4 without an environment map; GFX_ERR_INVALID_ARGUMENT for another op or a missing pointer. */
+int gfx_light_sample_debug(gfx_ctx* ctx, void* stream, int op, const float* params, const float* in, uint32_t n, float* out);
 /* test hook of the shading layer every renderer shares (BSDFs, sampling warps, encoders, frames); needs no scene.
  * material: 9 HOST floats {bsdfType, p0[3], p1[3], p2, regularize != 0}, read as setupBSDFBody reads a material with 1x1
  * textures (regularize = BSDFFlags::Regularize).  in / out: n DEVICE records of 8 floats each, unused output slots 0, integer

@@ -100,7 +100,9 @@ struct EnvLight {
     }
 };
 
-// RegularConstantContinuousDistribution1DTemplate::initialize, non-alias branch (common_host.cpp:292-312)
+// RegularConstantContinuousDistribution1DTemplate::initialize, non-alias branch (common_host.cpp:292-312).  Departure: with
+// integral 0 (a black row or map) the reference's lines compute 0 / 0 = NaN for every entry; here PDF = 0 and CDF = i / n
+// (DESIGN.md, "Environment maps with black rows").
 inline float buildRegularDistribution1D(const float* values, uint32_t n, float* PDF, float* CDF) {
     CompensatedSum sum;
     for (uint32_t i = 0; i < n; ++i) {
@@ -110,17 +112,27 @@ inline float buildRegularDistribution1D(const float* values, uint32_t n, float* 
     }
     const float integral = sum.result;
     for (uint32_t i = 0; i < n; ++i) {
-        PDF[i] /= integral;
-        CDF[i] /= integral;
+        if (integral > 0.0f) {
+            PDF[i] /= integral;
+            CDF[i] /= integral;
+        }
+        else {
+            PDF[i] = 0.0f;
+            CDF[i] = (float)i / (float)n;
+        }
     }
     CDF[n] = 1.0f;
     return integral;
 }
 
-inline void buildEnvLight(EnvLight* e, const float* rgba, uint32_t width, uint32_t height) {
+// false for a map with a NaN texel, which the clamp would pass into every pdf (the library refuses it the same way)
+inline bool buildEnvLight(EnvLight* e, const float* rgba, uint32_t width, uint32_t height) {
     *e = EnvLight();
     if (!rgba || !width || !height)
-        return;
+        return true;
+    for (size_t i = 0; i < (size_t)width * height; ++i)
+        if (std::isnan(rgba[4 * i]) || std::isnan(rgba[4 * i + 1]) || std::isnan(rgba[4 * i + 2]))
+            return false;
     e->W = width;
     e->H = height;
     e->texels.assign(rgba, rgba + 4 * (size_t)width * height);
@@ -144,6 +156,7 @@ inline void buildEnvLight(EnvLight* e, const float* rgba, uint32_t width, uint32
     e->topPdf.resize(height);
     e->topCdf.resize(height + 1);
     e->topIntegral = buildRegularDistribution1D(e->rowIntegral.data(), height, e->topPdf.data(), e->topCdf.data());
+    return true;
 }
 
 // one image texture of a material and tex2DLod<float4>(tex, u, v, 0) with the reference's material samplers

@@ -70,6 +70,7 @@ void orc_light_dist_export(orc_scene* s, float* instWeights, float* instCdf, flo
 /* environment light test hooks: op 0 sample (u0, u1) -> (u, v, uvPDF); 1 evaluatePDF(u, v); 2 texture fetch (u, v) -> rgb;
  * n pairs in, n triples out; -1 if the scene has no environment map */
 int orc_env_query(orc_scene* s, int op, const float* in, uint32_t n, float* out);
+int orc_light_sample_debug(orc_scene* s, int op, const float* params, const float* in, uint32_t n, float* out);
 
 orc_frame* orc_frame_create(orc_scene* s, uint32_t width, uint32_t height);
 void orc_frame_destroy(orc_frame* f);

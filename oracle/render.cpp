@@ -57,8 +57,11 @@ struct orc_scene {
     std::vector<uint32_t> materialTextures;  // ... [4 * m + k]: texture of p0 / p1 / p2 / emittance or 0xFFFFFFFF (empty = none)
 };
 
-// plp.s->envLightTexture && plp.f->enableEnvLight
-static inline bool useEnvLight(const orc_scene* s, const GfxFrameParams* p) { return s->env.present() && p->enableEnvLight; }
+// plp.s->envLightTexture && plp.f->enableEnvLight; a map that is black everywhere (importance integral 0) is no light to sample
+// and counts as none, as in the library (DESIGN.md, "Environment maps with black rows")
+static inline bool useEnvLight(const orc_scene* s, const GfxFrameParams* p) {
+    return s->env.present() && s->env.topIntegral > 0.0f && p->enableEnvLight;
+}
 
 // sequential fp32 exclusive scan (stands in for ext/cubd ExclusiveSum; SURVEY.md §8c item 4)
 static float exclusiveScan(const std::vector<float> &w, std::vector<float> &cdf) {
@@ -223,7 +226,10 @@ extern "C" orc_scene* orc_scene_create(const GfxSceneDesc* d, const OrcBuildConf
         s->instances[i].desc = d->instances[i];
     s->instanceMeshSlots.assign(d->instanceMeshSlots, d->instanceMeshSlots + d->numInstanceMeshSlots);
 
-    buildEnvLight(&s->env, d->envTexels, d->envWidth, d->envHeight);
+    if (!buildEnvLight(&s->env, d->envTexels, d->envWidth, d->envHeight)) { // a NaN texel: refused like gfx_scene_upload does
+        delete s;
+        return nullptr;
+    }
     if (d->materialTextures && d->numTextures) {
         s->textures.resize(d->numTextures);
         for (uint32_t t = 0; t < d->numTextures; ++t) {
@@ -827,8 +833,14 @@ extern "C" void orc_gbuffer(orc_frame* f, const GfxFrameParams* p, int numThread
 // ---------------------------------------------------------------------------------------
 static inline float convertToWeight(const float3 &c) { return (c.x + c.y + c.z) / 3; } // restir_di_shared.h:82-85
 
+// which light sampleLight picked, for the test hook orc_light_sample_debug: stage 0 / 1 = the instance / geometry early out, 2 = a
+// primitive; lightProb = the product of the three probabilities (set at stage 2 only)
+struct LightPickInfo {
+    uint32_t stage = 0, instSlot = 0, geomInstIndexInInst = 0, primIndex = 0;
+    float lightProb = 0.0f;
+};
 static void sampleLight(const orc_scene* s, const GfxFrameParams* p, float ul, bool sampleEnvLight, float u0, float u1,
-                        LightSample* lightSample, float* areaPDensity) {
+                        LightSample* lightSample, float* areaPDensity, LightPickInfo* pickInfo = nullptr) {
     // restir_di_shared.h:320-516, useSolidAngleSampling = false
     float3 emittance(0.0f);
     if (sampleEnvLight) { // :330-364
@@ -861,6 +873,8 @@ static void sampleLight(const orc_scene* s, const GfxFrameParams* p, float ul, b
     float instProb, uGeomInst;
     const uint32_t instSlot = lightInstDist.sample(ul, &instProb, &uGeomInst);
     lightProb *= instProb;
+    if (pickInfo)
+        pickInfo->instSlot = instSlot;
     const InstData &inst = s->instances[instSlot];
     if (instProb == 0.0f) {
         *areaPDensity = 0.0f;
@@ -873,6 +887,10 @@ static void sampleLight(const orc_scene* s, const GfxFrameParams* p, float ul, b
     const uint32_t geomInstSlot = s->instanceMeshSlots[inst.desc.firstMeshSlot + geomInstIndexInInst];
     lightProb *= geomInstProb;
     const MeshData &mesh = s->meshes[geomInstSlot];
+    if (pickInfo) {
+        pickInfo->stage = 1;
+        pickInfo->geomInstIndexInInst = geomInstIndexInInst;
+    }
     if (geomInstProb == 0.0f) {
         *areaPDensity = 0.0f;
         return;
@@ -882,6 +900,11 @@ static void sampleLight(const orc_scene* s, const GfxFrameParams* p, float ul, b
     float primProb;
     const uint32_t primIndex = emitterPrimDist.sample(uPrim, &primProb);
     lightProb *= primProb;
+    if (pickInfo) {
+        pickInfo->stage = 2;
+        pickInfo->primIndex = primIndex;
+        pickInfo->lightProb = lightProb;
+    }
 
     const GfxMaterialDesc &mat = s->materials[mesh.materialSlot];
     const uint32_t i0 = mesh.triangles[3 * primIndex], i1 = mesh.triangles[3 * primIndex + 1], i2 = mesh.triangles[3 * primIndex + 2];
@@ -914,6 +937,27 @@ static void sampleLight(const orc_scene* s, const GfxFrameParams* p, float ul, b
         emittance *= float3(mat.emittance[0], mat.emittance[1], mat.emittance[2]);
     }
     lightSample->emittance = emittance;
+}
+
+// the choice between the environment and the emitters that the streaming-RIS loops make for candidate i of n
+// (optix_restir_di_kernels.cu:74-90, build_cell_reservoirs.cu:120-139): the first probToSampleEnvLight * n candidates go to the
+// environment; returns sampleEnvLight and remaps ul
+static bool chooseEnvForCandidate(const orc_scene* s, const GfxFrameParams* p, uint32_t i, uint32_t numCandidates, float* ul,
+                                  float* probToSampleCurLightType) {
+    *probToSampleCurLightType = 1.0f;
+    if (!useEnvLight(s, p))
+        return false;
+    if (!(s->instIntegral > 0.0f))
+        return true;
+    const float prob = std::fmin(std::fmax(kProbToSampleEnvLight * numCandidates - i, 0.0f), 1.0f);
+    if (*ul < prob) {
+        *probToSampleCurLightType = kProbToSampleEnvLight;
+        *ul = *ul / prob;
+        return true;
+    }
+    *probToSampleCurLightType = 1.0f - kProbToSampleEnvLight;
+    *ul = (*ul - prob) / (1 - prob);
+    return false;
 }
 
 static bool evaluateVisibility(const orc_scene* s, const float3 &shadingPoint, const LightSample &ls) { // restir_di_shared.h:559-582
@@ -1054,25 +1098,8 @@ static void performInitialAndTemporalRIS(orc_frame* f, const GfxFrameParams* p, 
     const uint32_t numCandidates = 1u << p->log2NumCandidateSamples;
     for (uint32_t i = 0; i < numCandidates; ++i) {
         float ul = rng.getFloat0cTo1o();
-        float probToSampleCurLightType = 1.0f;
-        bool sampleEnvLight = false;
-        if (useEnvLight(s, p)) { // :74-90: the first probToSampleEnvLight * numCandidates candidates go to the environment
-            if (s->instIntegral > 0.0f) {
-                const float prob = std::fmin(std::fmax(kProbToSampleEnvLight * numCandidates - i, 0.0f), 1.0f);
-                if (ul < prob) {
-                    probToSampleCurLightType = kProbToSampleEnvLight;
-                    ul = ul / prob;
-                    sampleEnvLight = true;
-                }
-                else {
-                    probToSampleCurLightType = 1.0f - kProbToSampleEnvLight;
-                    ul = (ul - prob) / (1 - prob);
-                }
-            }
-            else {
-                sampleEnvLight = true;
-            }
-        }
+        float probToSampleCurLightType;
+        const bool sampleEnvLight = chooseEnvForCandidate(s, p, i, numCandidates, &ul, &probToSampleCurLightType);
         LightSample lightSample;
         float probDensity;
         const float u0 = rng.getFloat0cTo1o();
@@ -1442,4 +1469,96 @@ extern "C" void orc_restir(orc_frame* f, const GfxFrameParams* p, int pass, int 
 extern "C" uint64_t orc_restir_rearch(orc_frame* f, const GfxFrameParams* p, int pass, int numThreads) {
     if (numThreads <= 0) numThreads = omp_get_max_threads();
     return restirRearch(f, p, pass, numThreads);
+}
+
+// test hook of light sampling, the oracle's side of gfx_light_sample_debug (include/gfxb200.h) for ops 0 and 3-7: the same
+// records of 16 floats, params = {envLightRotation, envLightPowerCoeff, enableEnvLight != 0}.  Op 0's key is the library's light
+// record index (every triangle of every emissive geometry, in instance order) or its kPickNone code for an early out.
+extern "C" int orc_light_sample_debug(orc_scene* s, int op, const float* params, const float* in, uint32_t n, float* out) {
+    if (op < 0 || op > 7 || op == 1 || op == 2)
+        return -2;
+    if ((op == 3 || op == 4) && !s->env.present())
+        return -1;
+    GfxFrameParams p;
+    std::memset(&p, 0, sizeof(p));
+    p.envLightRotation = params[0];
+    p.envLightPowerCoeff = params[1];
+    p.enableEnvLight = params[2] != 0.0f ? 1u : 0u;
+    const uint32_t kPickNone = 0x40000000u;
+    std::vector<uint32_t> lightTriBase; // per flattened geometry, 0xFFFFFFFF for one without an emitter
+    uint32_t numLightTris = 0;
+    for (const InstData &inst : s->instances)
+        for (uint32_t k = 0; k < inst.desc.numMeshSlots; ++k) {
+            const MeshData &mesh = s->meshes[s->instanceMeshSlots[inst.desc.firstMeshSlot + k]];
+            lightTriBase.push_back(s->materials[mesh.materialSlot].hasEmittance ? numLightTris : 0xFFFFFFFFu);
+            if (s->materials[mesh.materialSlot].hasEmittance)
+                numLightTris += mesh.numTriangles;
+        }
+    std::vector<uint32_t> geomBase(s->instances.size());
+    for (size_t i = 0, g = 0; i < s->instances.size(); g += s->instances[i].desc.numMeshSlots, ++i)
+        geomBase[i] = (uint32_t)g;
+    auto bits = [](uint32_t u) { float f; std::memcpy(&f, &u, 4); return f; };
+    auto asUint = [](float f) { uint32_t u; std::memcpy(&u, &f, 4); return u; };
+#pragma omp parallel for schedule(static)
+    for (int64_t r = 0; r < (int64_t)n; ++r) {
+        const float* a = in + 16 * r;
+        float* o = out + 16 * r;
+        for (int k = 0; k < 16; ++k)
+            o[k] = 0.0f;
+        if (op == 0) {
+            LightSample ls;
+            ls.emittance = ls.position = ls.normal = float3(0.0f);
+            float density = 0.0f;
+            LightPickInfo pick;
+            sampleLight(s, &p, a[0], false, a[1], a[2], &ls, &density, &pick);
+            const InstData &inst = s->instances[pick.instSlot];
+            const uint32_t geomSlot = inst.desc.firstMeshSlot + pick.geomInstIndexInInst;
+            uint32_t key;
+            if (pick.stage == 0)
+                key = kPickNone | 0x20000000u | pick.instSlot;
+            else if (pick.stage == 1)
+                key = kPickNone | geomSlot;
+            else if (lightTriBase[geomBase[pick.instSlot] + pick.geomInstIndexInInst] == 0xFFFFFFFFu)
+                key = kPickNone | 0x10000000u | geomSlot;
+            else
+                key = lightTriBase[geomBase[pick.instSlot] + pick.geomInstIndexInInst] + pick.primIndex;
+            o[0] = bits(key);
+            o[1] = ls.position.x; o[2] = ls.position.y; o[3] = ls.position.z;
+            o[4] = ls.normal.x; o[5] = ls.normal.y; o[6] = ls.normal.z;
+            o[7] = ls.emittance.x; o[8] = ls.emittance.y; o[9] = ls.emittance.z;
+            o[10] = density;
+            o[11] = pick.lightProb;
+        }
+        else if (op == 3) {
+            LightSample ls;
+            ls.emittance = ls.position = ls.normal = float3(0.0f);
+            float density = 0.0f;
+            sampleLight(s, &p, 0.0f, true, a[0], a[1], &ls, &density);
+            o[0] = ls.position.x; o[1] = ls.position.y; o[2] = ls.position.z;
+            o[3] = density;
+            o[4] = ls.emittance.x; o[5] = ls.emittance.y; o[6] = ls.emittance.z;
+        }
+        else if (op == 4) {
+            const EnvMissTerms m = envMissTerms(s, &p, float3(a[0], a[1], a[2]), a[3], a[4]);
+            o[0] = m.hypAreaPDensity; o[1] = m.misWeight; o[2] = m.texCoord.x; o[3] = m.texCoord.y;
+        }
+        else if (op == 5) {
+            const uint32_t instSlot = asUint(a[0]), geomInInst = asUint(a[1]), primIndex = asUint(a[2]);
+            if (instSlot < s->instances.size() && geomInInst < s->instances[instSlot].desc.numMeshSlots) {
+                const InstData &inst = s->instances[instSlot];
+                const MeshData &mesh = s->meshes[s->instanceMeshSlots[inst.desc.firstMeshSlot + geomInInst]];
+                if (primIndex < mesh.numTriangles) {
+                    SurfacePoint sp;
+                    computeSurfacePointAtHit(s, &p, inst, mesh, primIndex, a[3], a[4], &sp);
+                    o[0] = sp.hypAreaPDensity;
+                }
+            }
+        }
+        else {
+            float ul = op == 6 ? a[2] : a[0], prob = 0.0f;
+            const bool env = op == 6 ? chooseEnvForCandidate(s, &p, asUint(a[0]), asUint(a[1]), &ul, &prob) : chooseEnvForNee(s, &p, &ul, &prob);
+            o[0] = env ? 1.0f : 0.0f; o[1] = ul; o[2] = prob;
+        }
+    }
+    return 0;
 }

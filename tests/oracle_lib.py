@@ -104,6 +104,8 @@ def lib() -> C.CDLL:
         L.orc_svgf_pass.argtypes = [vp, C.POINTER(abi.GfxFrameParams), C.c_int, C.c_uint32, C.c_int]
         L.orc_env_query.restype = C.c_int
         L.orc_env_query.argtypes = [vp, C.c_int, vp, C.c_uint32, vp]
+        L.orc_light_sample_debug.restype = C.c_int
+        L.orc_light_sample_debug.argtypes = [vp, C.c_int, vp, vp, C.c_uint32, vp]
         L.orc_rays_traced.restype = C.c_ulonglong
         L.orc_rays_traced.argtypes = [C.c_int]
         L.orc_nrc_create.restype = vp
@@ -144,7 +146,8 @@ class OracleScene:
         self.arrays = abi.SceneArrays(scene)
         self.cfg = cfg or reference_build_config()
         self.h = lib().orc_scene_create(C.byref(self.arrays.desc), C.byref(self.cfg), 0 if build_bvh else -1)
-        assert self.h
+        if not self.h:
+            raise ValueError("orc_scene_create refused the scene (an environment map with a NaN texel)")
 
     def close(self):
         if self.h:
@@ -160,6 +163,18 @@ class OracleScene:
         out = np.zeros((a.shape[0], 3), dtype=np.float32)
         rc = lib().orc_env_query(self.h, op, a.ctypes.data_as(C.c_void_p), a.shape[0], out.ctypes.data_as(C.c_void_p))
         assert rc == 0, "scene has no environment map"
+        return out
+
+    def light_sample_debug(self, op: int, records: np.ndarray, env_rotation: float = 0.0, env_power: float = 1.0,
+                           enable_env: bool = False) -> np.ndarray:
+        """the oracle's side of gfx_light_sample_debug, ops 0 and 3-7: records [n, <= 16] float32 -> [n, 16] float32"""
+        a = np.zeros((records.shape[0], 16), dtype=np.float32)
+        a[:, :records.shape[1]] = records
+        out = np.zeros_like(a)
+        params = (C.c_float * 3)(env_rotation, env_power, 1.0 if enable_env else 0.0)
+        rc = lib().orc_light_sample_debug(self.h, op, params, a.ctypes.data_as(C.c_void_p), a.shape[0],
+                                          out.ctypes.data_as(C.c_void_p))
+        assert rc == 0, f"orc_light_sample_debug({op}) = {rc}"
         return out
 
     def update_instances(self, instance_descs):
