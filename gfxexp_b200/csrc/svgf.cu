@@ -553,6 +553,12 @@ DevSvgf makeDevSvgf(const gfx_ctx* ctx, const GfxFrameParams* params) {
 } // namespace
 
 int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int pass, uint32_t stage) {
+    // The depth gradient of both filters reads the neighbour x + (x < W/2 ? 1 : -1) and row y + (y < H/2 ? 1 : -1): pixel -1 and
+    // row -1 on frames one pixel wide or high, as in the reference (svgf.cu:75-78, 268-271).  Such frames are refused.
+    if ((pass == GFX_SVGF_ESTIMATE_VARIANCE || pass == GFX_SVGF_ATROUS) && (ctx->frame.W < 2 || ctx->frame.H < 2)) {
+        ctx->setError("gfx_svgf_launch: the variance and à-trous passes need a frame of at least 2x2 pixels");
+        return GFX_ERR_INVALID_ARGUMENT;
+    }
     bool jitter;
     float2 sample;
     const int rc = svgfSubPixelSample(ctx, params, &jitter, &sample);

@@ -529,12 +529,16 @@ void modulateAndTAA(orc_svgf* s, const GfxFrameParams* p, uint32_t numFilteringS
 
 } // namespace
 
-extern "C" void orc_svgf_pass(orc_svgf* s, const GfxFrameParams* p, int pass, uint32_t stage, int numThreads) {
+// Returns GFX_ERR_INVALID_ARGUMENT, and runs nothing, for the variance and à-trous passes on a frame narrower or shorter than
+// 2 pixels, whose depth-gradient neighbour lies outside the frame (gfx_svgf_launch refuses them alike); GFX_OK otherwise.
+extern "C" int orc_svgf_pass(orc_svgf* s, const GfxFrameParams* p, int pass, uint32_t stage, int numThreads) {
+    const int W = (int)s->W, H = (int)s->H;
+    if ((pass == GFX_SVGF_ESTIMATE_VARIANCE || pass == GFX_SVGF_ATROUS) && (W < 2 || H < 2))
+        return GFX_ERR_INVALID_ARGUMENT;
     if (numThreads <= 0) numThreads = omp_get_max_threads();
     const View v = makeView(s->frame);
     const Cam cam = makeCam(p->camera);
     const Cam prevCam = makeCam(p->prevCamera);
-    const int W = (int)s->W, H = (int)s->H;
     const int y0 = (int)p->tileOriginY, y1 = p->tileRows ? std::min(H, (int)(p->tileOriginY + p->tileRows)) : H;
 #pragma omp parallel for schedule(dynamic, 4) num_threads(numThreads)
     for (int y = y0; y < y1; ++y) {
@@ -549,4 +553,5 @@ extern "C" void orc_svgf_pass(orc_svgf* s, const GfxFrameParams* p, int pass, ui
             }
         }
     }
+    return GFX_OK;
 }

@@ -15,7 +15,7 @@
 #include "svgf_app.cpp"
 
 extern "C" {
-void orc_svgf_pass(orc_svgf* s, const GfxFrameParams* p, int pass, uint32_t stage, int numThreads); // denoise.cpp
+int orc_svgf_pass(orc_svgf* s, const GfxFrameParams* p, int pass, uint32_t stage, int numThreads); // denoise.cpp
 }
 
 extern "C" void orc_svgf_subpixel_offset(uint32_t i, float* offset) {

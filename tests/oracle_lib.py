@@ -101,6 +101,7 @@ def lib() -> C.CDLL:
         L.orc_svgf_destroy.argtypes = [vp]
         L.orc_svgf_buffer_ptr.restype = vp
         L.orc_svgf_buffer_ptr.argtypes = [vp, C.c_int, C.c_uint32, C.POINTER(C.c_size_t)]
+        L.orc_svgf_pass.restype = C.c_int
         L.orc_svgf_pass.argtypes = [vp, C.POINTER(abi.GfxFrameParams), C.c_int, C.c_uint32, C.c_int]
         L.orc_env_query.restype = C.c_int
         L.orc_env_query.argtypes = [vp, C.c_int, vp, C.c_uint32, vp]
@@ -261,12 +262,14 @@ class OracleFrame:
     def __del__(self):
         self.close()
 
-    def buffer(self, buffer_id: int, index: int = 0) -> np.ndarray:
+    def buffer(self, buffer_id: int, index: int = 0, copy: bool = True) -> np.ndarray:
+        """copy=False returns a writable view of the oracle's memory"""
         nbytes = C.c_size_t()
         ptr = lib().orc_buffer_ptr(self.h, buffer_id, index, C.byref(nbytes))
         dtype, comps, planes = abi.BUFFER_LAYOUT[buffer_id]
         raw = (C.c_uint8 * nbytes.value).from_address(ptr)
-        arr = np.frombuffer(raw, dtype=dtype).copy()
+        arr = np.frombuffer(raw, dtype=dtype)
+        arr = arr.copy() if copy else arr
         if planes > 1:
             return arr.reshape(planes, self.H, self.W, comps)
         return arr.reshape(self.H, self.W, comps) if comps > 1 else arr.reshape(self.H, self.W)
@@ -352,15 +355,18 @@ class OracleSvgf:
     def __del__(self):
         self.close()
 
-    def run(self, params, pass_id: int, stage: int = 0, threads: int = 0):
-        lib().orc_svgf_pass(self.h, C.byref(params), pass_id, stage, threads)
+    def run(self, params, pass_id: int, stage: int = 0, threads: int = 0) -> int:
+        """GFX_OK, or GFX_ERR_INVALID_ARGUMENT (-1) for the variance and a-trous passes on a frame under 2x2 pixels"""
+        return lib().orc_svgf_pass(self.h, C.byref(params), pass_id, stage, threads)
 
-    def buffer(self, buffer_id: int, index: int = 0) -> np.ndarray:
+    def buffer(self, buffer_id: int, index: int = 0, copy: bool = True) -> np.ndarray:
+        """copy=False returns a writable view of the oracle's memory"""
         nbytes = C.c_size_t()
         ptr = lib().orc_svgf_buffer_ptr(self.h, buffer_id, index, C.byref(nbytes))
         dtype, comps, planes = abi.BUFFER_LAYOUT[buffer_id]
         raw = (C.c_uint8 * nbytes.value).from_address(ptr)
-        arr = np.frombuffer(raw, dtype=dtype).copy()
+        arr = np.frombuffer(raw, dtype=dtype)
+        arr = arr.copy() if copy else arr
         return arr.reshape(self.H, self.W, comps) if comps > 1 else arr.reshape(self.H, self.W)
 
 
