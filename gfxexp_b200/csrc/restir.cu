@@ -422,7 +422,7 @@ __global__ void __launch_bounds__(64) k_spatialRIS(DevScene s, DevFrame f, DevFr
                 if (useUnbiasedEstimator)
                     selectedNeighborIndex = nIdx;
             }
-            combinedStreamLength += nbStreamLength;
+            combinedStreamLength = saturatedStreamLength(combinedStreamLength, nbStreamLength);
         }
     }
     combinedReservoir.streamLength = combinedStreamLength;

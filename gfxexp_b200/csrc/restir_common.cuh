@@ -43,6 +43,11 @@ GFX_D void storeReservoir(const DevFrame &f, uint32_t idx, size_t pix, const Res
     f.reservoir[idx][2 * n + pix] = make_float4(r.sample.normal.x, r.sample.normal.y, r.sample.normal.z, 0.0f);
 }
 
+// M is kept in 31 bits next to atInfinity.  Spatial passes add up to 16 stream lengths per pass and any number of passes may
+// run, so the sum saturates at 2^31 - 1 instead of wrapping into atInfinity (the reference keeps a full uint32_t, which
+// wraps at 2^32).  Both inputs are at most 2^31 - 1, so the 32-bit sum cannot wrap.
+GFX_D uint32_t saturatedStreamLength(uint32_t a, uint32_t b) { return min(a + b, 0x7FFFFFFFu); }
+
 template <bool testGeometry>
 GFX_D bool testNeighbor(const DevFrame &f, const DevCamera &camera, uint32_t nbBufIdx, int nbx, int nby, float dist,
                         const f3 &normalInWorld) { // restir_di_shared.h:747-771

@@ -1020,6 +1020,11 @@ static inline void storeReservoir(orc_frame* f, uint32_t idx, size_t pix, const 
     f->reservoir[idx][2 * n + pix] = F4{ r.sample.normal.x, r.sample.normal.y, r.sample.normal.z, 0.0f };
 }
 
+// The reservoir planes keep M in 31 bits next to atInfinity.  Spatial passes add up to 16 stream lengths per pass and any
+// number of passes may run, so the sum saturates at 2^31 - 1 instead of wrapping into atInfinity.  Both inputs are at most
+// 2^31 - 1, so the 32-bit sum cannot wrap.
+static inline uint32_t saturatedStreamLength(uint32_t a, uint32_t b) { return std::min(a + b, 0x7FFFFFFFu); }
+
 template <bool testGeometry>
 static bool testNeighbor(const orc_frame* f, const Camera &camera, uint32_t nbBufIdx, int nbx, int nby, float dist, const float3 &normalInWorld) {
     // restir_di_shared.h:747-771
@@ -1300,7 +1305,7 @@ static void performSpatialRIS(orc_frame* f, const GfxFrameParams* p, const Camer
                 if (useUnbiasedEstimator)
                     selectedNeighborIndex = nIdx;
             }
-            combinedStreamLength += nbStreamLength;
+            combinedStreamLength = saturatedStreamLength(combinedStreamLength, nbStreamLength);
         }
     }
     combinedReservoir.streamLength = combinedStreamLength;
