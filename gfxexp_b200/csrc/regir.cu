@@ -57,8 +57,9 @@ void regirGrid(const GfxFrameParams* p, uint32_t dim[3], float origin[3], float 
     }
 }
 
-// initializeReservoirs (regir_main.cpp:1073-1095)
-static int ensureRegir(gfx_ctx* ctx, const GfxFrameParams* p) {
+// initializeReservoirs (regir_main.cpp:1073-1112), run by the build of frame `frameIndex` whenever the grid is new: the
+// frame's first build, a build after gfx_frame_create, or a new regirGridDim
+static int ensureRegir(gfx_ctx* ctx, const GfxFrameParams* p, uint32_t frameIndex) {
     FrameState::Regir &R = ctx->frame.regir;
     uint32_t dim[3];
     float origin[3], cellSize[3];
@@ -80,8 +81,11 @@ static int ensureRegir(gfx_ctx* ctx, const GfxFrameParams* p) {
     GFX_CUDA(ctx, cudaMalloc(&R.lastAccessFrameIndices, (size_t)R.numCells * 4));
     GFX_CUDA(ctx, cudaMalloc(&R.numActiveCells, 8));
     GFX_CUDA(ctx, cudaMemset(R.perCellNumAccesses, 0, (size_t)R.numCells * 4));
-    GFX_CUDA(ctx, cudaMemset(R.lastAccessFrameIndices, 0xFF, (size_t)R.numCells * 4)); // fill(frameIndex = -1)
     GFX_CUDA(ctx, cudaMemset(R.numActiveCells, 0, 8));
+    // the reference fills with -1 at startup (frame 0); frameIndex - 1 keeps that there and, for a grid created later, keeps
+    // every cell built for the next 8 frames as well instead of idle from the start (DESIGN.md)
+    const std::vector<uint32_t> lastAccess(R.numCells, frameIndex - 1u);
+    GFX_CUDA(ctx, cudaMemcpy(R.lastAccessFrameIndices, lastAccess.data(), lastAccess.size() * 4, cudaMemcpyHostToDevice));
     std::vector<unsigned long long> states(R.numSlots);
     std::mt19937_64 rngSeed(591842031321323413ull);
     for (auto &st : states)
@@ -187,7 +191,9 @@ __global__ void __launch_bounds__(128) k_regirBuildCells(DevScene s, DevRegir rg
         const f3 cont = sampleIntensity(s, cellCenter, halfCellSize, minSquaredDistance, uLight, sampleEnv, uPos0, uPos1, &lightSample, &areaPDensity);
         areaPDensity *= probToSampleCurLightType;
         const float targetPDensity = convertToWeight(cont);
-        const float weight = targetPDensity / areaPDensity;
+        // a sample its sampler cannot produce (the environment's poles, areaPDensity = 0) weighs 0 rather than the
+        // reference's 0 / 0 = NaN, which the temporal merge would carry in sumWeights forever (DESIGN.md)
+        const float weight = areaPDensity > 0.0f ? targetPDensity / areaPDensity : 0.0f;
         if (reservoir.update(lightSample, weight, rng.getFloat0cTo1o()))
             selectedTargetPDensity = targetPDensity;
     }
@@ -216,7 +222,8 @@ __global__ void __launch_bounds__(128) k_regirBuildCells(DevScene s, DevRegir rg
         const float prevTargetDensity = p3.x;
         const uint32_t prevStreamLength = min(prevM, maxNumPrevSamples);
         const float lengthCorrection = static_cast<float>(prevStreamLength) / prevM;
-        const float weight = lengthCorrection * p0.w;
+        // a slot that was never built (M = 0) weighs 0 rather than the reference's 0 / 0 = NaN (DESIGN.md)
+        const float weight = prevM > 0 ? lengthCorrection * p0.w : 0.0f;
         if (reservoir.update(prevLightSample, weight, rng.getFloat0cTo1o()))
             selectedTargetPDensity = prevTargetDensity;
         combinedStreamLength += prevStreamLength;
@@ -250,7 +257,7 @@ __global__ void k_regirUpdateAccess(DevRegir rg, uint32_t frameIndex) {
 }
 
 int launchRegirBuildCells(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, uint32_t frameIndex, int useTemporalReuse) {
-    const int rc = ensureRegir(ctx, params);
+    const int rc = ensureRegir(ctx, params, frameIndex);
     if (rc != GFX_OK)
         return rc;
     if (!ctx->scene.uploaded) {

@@ -534,7 +534,9 @@ static void regirPathTracePixelBump(orc_frame* f, orc_regir* r, const GfxFramePa
 }
 
 static uint64_t regirPathTraceBump(orc_frame* f, const GfxFrameParams* p, int numThreads) {
-    orc_regir* r = regirState(f, p);
+    orc_regir* r = f->regir;
+    if (!r)
+        return ORC_NOT_READY;
     const Camera camera = makeCamera(p->camera);
     const uint32_t W = f->W, H = f->H;
     const uint32_t y0 = p->tileOriginY, y1 = p->tileRows ? std::min(H, p->tileOriginY + p->tileRows) : H;

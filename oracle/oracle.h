@@ -86,6 +86,8 @@ void orc_present(const float* srcRGBA, uint32_t width, uint32_t height, const Gf
 void orc_gbuffer(orc_frame* f, const GfxFrameParams* p, int numThreads);
 void orc_restir(orc_frame* f, const GfxFrameParams* p, int pass, int numThreads);
 /* unidirectional path tracer (GfxPathTraceVariant); returns the number of rays traced */
+// GFX_PT_REGIR before a ReGIR build returns ORC_NOT_READY (the library returns GFX_ERR_NOT_READY) and writes nothing
+#define ORC_NOT_READY UINT64_MAX
 uint64_t orc_pathtrace(orc_frame* f, const GfxFrameParams* p, int variant, int numThreads);
 /* rearchitected ReSTIR passes GFX_RESTIR_PRESAMPLE_LIGHTS .. GFX_RESTIR_SHADE_AND_RESAMPLE; returns shadow rays traced */
 uint64_t orc_restir_rearch(orc_frame* f, const GfxFrameParams* p, int pass, int numThreads);

@@ -15,6 +15,7 @@ import numpy as np
 
 from gfxexp_b200 import abi
 from tests import oracle_lib
+from tests.oracle_lib import ORC_NOT_READY
 
 LIB = os.path.join(oracle_lib.ORACLE_DIR, "liborc_bump.so")
 _lib = None
@@ -136,7 +137,10 @@ class OracleFrame:
         return int(lib().orc_restir_rearch(self.h, C.byref(params), pass_id, threads))
 
     def pathtrace(self, params, variant: int = 0, threads: int = 0) -> int:
-        return int(lib().orc_bump_pathtrace(self.h, C.byref(params), variant, threads))
+        rays = int(lib().orc_bump_pathtrace(self.h, C.byref(params), variant, threads))
+        if rays == ORC_NOT_READY:
+            raise RuntimeError("orc_bump_pathtrace(GFX_PT_REGIR): call regir_build_cells first")
+        return rays
 
     def regir_build_cells(self, params, frame_index: int, temporal: bool, threads: int = 0):
         lib().orc_regir_build_cells(self.h, C.byref(params), frame_index & 0xFFFFFFFF, 1 if temporal else 0, threads)

@@ -16,6 +16,7 @@ from gfxexp_b200 import abi
 _ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ORACLE_DIR = os.path.join(_ROOT, "oracle")
 ORACLE_LIB = os.path.join(ORACLE_DIR, "liboracle.so")
+ORC_NOT_READY = (1 << 64) - 1   # orc_pathtrace(GFX_PT_REGIR) before a ReGIR build (oracle.h)
 
 
 class OrcBuildConfig(C.Structure):
@@ -282,7 +283,10 @@ class OracleFrame:
 
     def pathtrace(self, params, variant: int = 0, threads: int = 0) -> int:
         """one sample per pixel of the path tracer; returns the number of rays traced"""
-        return int(lib().orc_pathtrace(self.h, C.byref(params), variant, threads))
+        rays = int(lib().orc_pathtrace(self.h, C.byref(params), variant, threads))
+        if rays == ORC_NOT_READY:
+            raise RuntimeError("orc_pathtrace(GFX_PT_REGIR): call regir_build_cells first")
+        return rays
 
 
     # -- NRC frame (nrc_setup_kernels.cu) -----------------------------------------------------------

@@ -32,12 +32,12 @@ def _normal(cls):
     return TILTED if cls else UP
 
 
-def gbuffers(W, H, mat=S.DS3, checker=False) -> dict:
+def gbuffers(W, H, mat=S.DS3, checker=False, point=POINT) -> dict:
     yy, xx = np.mgrid[0:H, 0:W]
     cls = ((xx + yy) % 2 == 1) if checker else np.zeros((H, W), bool)
     gb0 = np.zeros((H, W, 4), np.uint32)
     gb2 = np.zeros((H, W, 4), np.uint32)
-    gb2[..., :3] = POINT.astype(np.float32).view(np.uint32)
+    gb2[..., :3] = np.asarray(point).astype(np.float32).view(np.uint32)
     gb2[..., 3] = S.encode(UP[None])[0]
     gb3 = np.zeros((H, W, 4), np.uint32)
     for c in (0, 1):
@@ -56,9 +56,10 @@ def _repeat(sp, n):
     return pts
 
 
-def integral(s64, cam, mat=S.DS3, cls=0, n=96, k=16, env_power=1.0, env_rotation=0.0):
-    """float64 direct lighting of the shading point of class cls seen from cam"""
-    g, _ = gbuffers(1, 2, mat, True)
+def integral(s64, cam, mat=S.DS3, cls=0, n=96, k=16, env_power=1.0, env_rotation=0.0, point=POINT, mask=None):
+    """float64 direct lighting of the shading point of class cls seen from cam; mask(position, normal) -> bool, if given,
+    keeps only the emitter points it accepts"""
+    g, _ = gbuffers(1, 2, mat, True, point)
     gb = {i: v[cls:cls + 1] for i, v in zip(range(4), g.values())}
     sp = restir_ref.ShadingPoints(s64, gb, np.array([0]), cam)
     i, j = np.meshgrid(np.arange(n), np.arange(n), indexing="ij")
@@ -75,6 +76,8 @@ def integral(s64, cam, mat=S.DS3, cls=0, n=96, k=16, env_power=1.0, env_rotation
         nrm = nrm @ em.normal_matrix[t].T
         nrm /= np.linalg.norm(nrm, axis=-1, keepdims=True)
         cont, _ = pts.direct(pos, nrm, np.broadcast_to(em.emittance[t], pos.shape), np.zeros(len(a), bool), True)
+        if mask is not None:
+            cont = cont * mask(pos, nrm)[:, None]
         total += cont.sum(0) * em.area_world[t] / n ** 2
     env = getattr(s64.scene, "env_map", None)
     if env is not None:
