@@ -253,35 +253,24 @@ struct NrcVertexRequest {
     bool fromRayGen;
 };
 
-// queues the rays of a vertex like emitRays() and, for a training path, stages its training vertex
+// queues the rays of a vertex with emitRays() and, for a training path, stages its training vertex; the shadow ray carries
+// the vertex's NEE estimate to NrcShadowWriter
 GFX_D void emitRaysNrc(const DevScene &s, const DevPathState &ps, const DevNrc &n, uint32_t* roundCounters, uint32_t nextQueue,
                        uint32_t lane, uint32_t pix, const f3 &positionInWorld, const VertexOutput &v, bool alive,
                        const NrcVertexRequest &req) {
-    const bool wantShadow = alive && v.wantShadow;
-    const bool wantExt = alive && v.wantExtension;
-    const uint32_t shadowSlot = allocQueueSlot(roundCounters + 2, wantShadow, lane);
-    const uint32_t extSlot = allocQueueSlot(roundCounters + 0, wantExt, lane);
-    if (wantShadow) {
-        ps.shadowRays[2 * (size_t)shadowSlot] = make_float4(positionInWorld.x, positionInWorld.y, positionInWorld.z, 0.0f);
-        ps.shadowRays[2 * (size_t)shadowSlot + 1] = make_float4(v.shadowDir.x, v.shadowDir.y, v.shadowDir.z, v.shadowTmax);
-        ps.shadowPixel[shadowSlot] = pix;
-        ps.shadowPending[shadowSlot] = v.pending;
-        n.shadowPending2[shadowSlot] = make_float4(v.neeUnoccluded.x, v.neeUnoccluded.y, v.neeUnoccluded.z,
-                                                   __uint_as_float(alive && req.wantVertex ? req.tile : 0xFFFFFFFFu));
-    }
-    if (wantExt) {
-        ps.extRays[nextQueue][2 * (size_t)extSlot] = make_float4(positionInWorld.x, positionInWorld.y, positionInWorld.z, 0.0f);
-        ps.extRays[nextQueue][2 * (size_t)extSlot + 1] = make_float4(v.nextDir.x, v.nextDir.y, v.nextDir.z, 3.402823466e+38f);
-        ps.extPixel[nextQueue][extSlot] = pix;
-    }
-    if (alive && req.wantVertex) {
-        n.stagedFlags[req.tile] = 1u | (req.fromRayGen ? 2u : 0u) | (req.pathLength << 8);
-        n.stagedThroughput[req.tile] = make_float4(v.localThroughput.x, v.localThroughput.y, v.localThroughput.z, 0.0f);
-        n.stagedNEE[req.tile] = make_float4(v.directContNEE.x, v.directContNEE.y, v.directContNEE.z, 0.0f);
-    }
-    const uint32_t cnt = __popc(__ballot_sync(0xFFFFFFFFu, wantShadow)) + __popc(__ballot_sync(0xFFFFFFFFu, wantExt));
-    if (lane == 0 && cnt)
-        atomicAdd(s.rayCounter, (unsigned long long)cnt);
+    emitRays(
+        s, ps, roundCounters, nextQueue, lane, pix, positionInWorld, v, alive,
+        [&](uint32_t shadowSlot) {
+            n.shadowPending2[shadowSlot] = make_float4(v.neeUnoccluded.x, v.neeUnoccluded.y, v.neeUnoccluded.z,
+                                                       __uint_as_float(alive && req.wantVertex ? req.tile : 0xFFFFFFFFu));
+        },
+        [&] {
+            if (alive && req.wantVertex) {
+                n.stagedFlags[req.tile] = 1u | (req.fromRayGen ? 2u : 0u) | (req.pathLength << 8);
+                n.stagedThroughput[req.tile] = make_float4(v.localThroughput.x, v.localThroughput.y, v.localThroughput.z, 0.0f);
+                n.stagedNEE[req.tile] = make_float4(v.directContNEE.x, v.directContNEE.y, v.directContNEE.z, 0.0f);
+            }
+        });
 }
 
 // pathTrace_raygen_generic<true> up to the path extension loop (optix_pathtracing_kernels.cu:95-283).  BUMP:
@@ -322,32 +311,27 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrame
         f3 radiance(0.001f, 0.001f, 0.001f);
         if (gb0.x != 0xFFFFFFFFu) {
             flags |= NRC_F_PRIMARY_HIT;
-            const DevInstance* inst = s.instances + gb0.x;
-            const DevMesh mesh = s.meshes[gb0.y];
-            const float bcB = decodeBarycentric((uint16_t)(gb0.w & 0xFFFFu));
-            const float bcC = decodeBarycentric((uint16_t)(gb0.w >> 16));
-            SurfacePoint sp;
-            computeSurfacePointFromGBuffer(s, inst, mesh, gb0.z, bcB, bcC, &sp);
-
+            GBufferHit h;
+            decodeGBufferHit(s, gb0, &h);
             const f3 alpha(1.0f);
             PCG32RNG rng{ f.rng[pix] };
-            const GfxMaterialDesc* mat = s.materials + mesh.materialSlot;
-            f3 vOut = p.camera.position - sp.positionInWorld;
+            const GfxMaterialDesc* mat = s.materials + h.mesh.materialSlot;
+            f3 vOut = p.camera.position - h.sp.positionInWorld;
             const float primaryDist2 = sqLength(vOut);
             vOut /= sqrtf(primaryDist2);
-            const float primaryDotVN = dot(vOut, sp.geometricNormalInWorld);
+            const float primaryDotVN = dot(vOut, h.sp.geometricNormalInWorld);
             const float frontHit = primaryDotVN >= 0.0f ? 1.0f : -1.0f;
-            positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
+            positionInWorld = offsetRayOrigin(h.sp.positionInWorld, frontHit * h.sp.geometricNormalInWorld);
             primaryPathSpread = primaryDist2 / (4 * kPi * fabsf(primaryDotVN));
-            ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+            ReferenceFrame shadingFrame(h.sp.shadingNormalInWorld, h.sp.texCoord0DirInWorld);
             if (BUMP) // :182-185
-                shadingFrame = bumpShadingFrameAtHit(s, mesh, gb0.z, bcB, bcC, shadingFrame);
+                shadingFrame = bumpShadingFrameAtHit(s, h.mesh, gb0.z, h.bcB, h.bcC, shadingFrame);
             const f3 vOutLocal = shadingFrame.toLocal(vOut);
 
             radiance = f3(0.0f);
             if (vOutLocal.z > 0 && mat->hasEmittance)
                 radiance += alpha * f3(mat->emittance[0], mat->emittance[1], mat->emittance[2]) / kPi;
-            const BSDF bsdf = setupBsdfAtHit(s, mesh, gb0.z, bcB, bcC);
+            const BSDF bsdf = setupBsdfAtHit(s, h.mesh, gb0.z, h.bcB, h.bcC);
             shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, &radiance, &v);
             f.rng[pix] = rng.state;
             ps.alphaPdf[pix] = make_float4(v.alpha.x, v.alpha.y, v.alpha.z, v.dirPDensity);
@@ -410,13 +394,7 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
             do {
                 if (hit.y == 0xFFFFFFFFu) { // pathTrace_miss_generic (:625-672): implicit environment light, MIS
                     if (s.env.enabled) {
-                        const float4 r1 = ps.extRays[curQueue][2 * (size_t)slot + 1];
-                        const float4 ap = ps.alphaPdf[pix];
-                        const f3 directContImplicit = evaluateEnvLightOnMiss(s, f3(r1.x, r1.y, r1.z), ap.w, true);
-                        float4 rad = ps.radiance[pix];
-                        const f3 add = f3(ap.x, ap.y, ap.z) * directContImplicit;
-                        rad.x += add.x; rad.y += add.y; rad.z += add.z;
-                        ps.radiance[pix] = rad;
+                        const f3 directContImplicit = addEnvLightOnMiss(s, ps, curQueue, slot, pix, true);
                         const uint32_t prevTrainDataIndex = isTrainingPath ? n.tilePrev[tile] : kInvalidVertexDataIndex;
                         if (isTrainingPath && prevTrainDataIndex != kInvalidVertexDataIndex) {
                             const float4 pb = n.pathB[pix];
@@ -439,20 +417,12 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
                 const uint32_t prevTrainDataIndex = isTrainingPath ? n.tilePrev[tile] : kInvalidVertexDataIndex;
                 bool trainingSuffixEndsWithCache = isTrainingPath ? n.tileSuffixEnded[tile] != 0 : false;
 
-                const uint2 im = __ldg(s.geomToInstMesh + hit.x);
-                const DevInstance* inst = s.instances + im.x;
-                const DevMesh mesh = s.meshes[im.y];
-                SurfacePoint sp;
-                computeSurfacePointAtHit(s, inst, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), &sp);
-                const GfxMaterialDesc* mat = s.materials + mesh.materialSlot;
-
-                const f3 vOut = normalize(-rayDir);
-                const float frontHit = dot(vOut, sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
-                ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
-                if (BUMP) // :398-401
-                    shadingFrame = bumpShadingFrameAtHit(s, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), shadingFrame);
-                positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
-                const f3 vOutLocal = shadingFrame.toLocal(vOut);
+                HitVertex h;
+                setupHitVertex<BUMP>(s, hit, rayDir, &h);
+                const f3 &vOut = h.vOut, &vOutLocal = h.vOutLocal;
+                const ReferenceFrame &shadingFrame = h.shadingFrame;
+                positionInWorld = h.positionInWorld;
+                const GfxMaterialDesc* mat = s.materials + h.mesh.materialSlot;
 
                 const float dist2 = sqLength(positionInWorld - rayOrigin);
                 curSqrtPathSpread += sqrtf(dist2 / (prevDirPDensity * fabsf(vOutLocal.z)));
@@ -463,13 +433,10 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
                     ps.radiance[pix] = make_float4(radiance.x, radiance.y, radiance.z, 0.0f);
                 };
 
-                // implicit light sampling (:417-445)
+                // implicit light sampling (:417-445), alpha * (emittance * w)
                 if (vOutLocal.z > 0 && mat->hasEmittance) {
                     const f3 emittance(mat->emittance[0], mat->emittance[1], mat->emittance[2]);
-                    const float lightPDensity = sp.hypAreaPDensity * dist2 / vOutLocal.z;
-                    const float bsdfPDensity = prevDirPDensity;
-                    const float misWeight = pow2f(bsdfPDensity) / (pow2f(bsdfPDensity) + pow2f(lightPDensity));
-                    const f3 directContImplicit = emittance * (misWeight / kPi);
+                    const f3 directContImplicit = emittance * implicitEmissionWeight(h.sp.hypAreaPDensity, dist2, vOutLocal.z, prevDirPDensity);
                     radiance += alpha * directContImplicit;
                     if (isTrainingPath && prevTrainDataIndex != kInvalidVertexDataIndex) {
                         const float4 pb = n.pathB[pix];
@@ -497,7 +464,7 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
                     recContinueProb = 1.0f / continueProb;
                 }
 
-                const BSDF bsdf = setupBsdfAtHit(s, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w));
+                const BSDF bsdf = setupBsdfAtHit(s, h.mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w));
 
                 // termination into the cache by the spread heuristic (:474-531)
                 bool endsWithCache = pow2f(curSqrtPathSpread) > kPathTerminationFactor * primaryPathSpread;
@@ -755,60 +722,43 @@ int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* 
     // a training path is exempt from Russian roulette at pathLength 2 (:452-453), so even maxPathLength <= 2 needs
     // the round with pathLength 3
     const uint32_t numRounds = (maxPathLength > 0 ? min(max(maxPathLength, 3u), kMaxNrcRounds) : kMaxNrcRounds) - 1u;
-    GFX_CUDA(ctx, cudaMemsetAsync(F.ptCounters, 0, (kMaxPathRounds + 1) * 16, stream));
-
-    const dim3 block(8, 8);
-    const dim3 grid((F.W + 7) / 8, (p.y1 - p.y0 + 7) / 8);
     const uint32_t scatterGrid = (n.numSuffixes + 127) / 128;
     int commitError = 0;
-    auto commit = [&]() {
-        GFX_TIMED(ctx, stream, "nrc_commit");
-        k_nrcCommitScan<<<1, 1024, 0, stream>>>(n, p.bufferIndex, F.W, F.H);
-        if (sharded) // one word per rank and round: the only exchange the path tracer needs
-            commitError |= allGather(n.shardCounts + 64, n.shardCounts, 1, 3 /* ncclUint32 */, F.nrc.shardComm, stream);
-        k_nrcCommitScatter<<<scatterGrid, 128, 0, stream>>>(n, numPixels, p.bufferIndex);
-        ctx->launches += 2;
-        if (sharded) {
-            k_nrcCommitAdvance<<<1, 1, 0, stream>>>(n, p.bufferIndex);
-            ctx->launches++;
-        }
-    };
     const bool bump = params->enableBumpMapping != 0;
-    { GFX_TIMED(ctx, stream, "nrc_first_hit");
-    if (bump)
-        k_nrcFirstHit<true><<<grid, block, 0, stream>>>(s, f, p, ps, n);
-    else
-        k_nrcFirstHit<false><<<grid, block, 0, stream>>>(s, f, p, ps, n); }
-    commit();
-    ctx->launches += 1;
-    const int traceGrid = wavefrontGrid();
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
-    const NrcShadowWriter shadowWriter{ ps.shadowPixel, ps.shadowPending, n.shadowPending2, ps.radiance, n.stagedIndex, n.trainTarget[0] };
-    const ExtensionHitWriter extWriter{ ps.extHits };
-    for (uint32_t round = 0; round < numRounds; ++round) {
-        uint32_t* c = F.ptCounters + 4 * round;
-        { GFX_TIMED(ctx, stream, "nrc_trace_shadow"); k_traceWavefront<true, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.shadowRays, c + 2, 0u, c + 3, shadowWriter); }
-        { GFX_TIMED(ctx, stream, "nrc_trace_extension"); k_traceWavefront<false, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.extRays[round & 1], c + 0, 0u, c + 1, extWriter); }
-        { GFX_TIMED(ctx, stream, "nrc_bounce");
-        if (bump)
-            k_nrcBounce<true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, n, round);
-        else
-            k_nrcBounce<false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, n, round); }
-        commit();
-        ctx->launches += 3;
-    }
-    // shadow rays requested by the last round (a training path may still have sampled a light there)
-    {
-        uint32_t* c = F.ptCounters + 4 * numRounds;
-        k_traceWavefront<true, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.shadowRays, c + 2, 0u, c + 3, shadowWriter);
-        ctx->launches++;
-    }
-    const uint32_t firstPixel = p.y0 * F.W, endPixel = p.y1 * F.W;
-    { GFX_TIMED(ctx, stream, "nrc_finish");
-    k_nrcFinish<<<(endPixel - firstPixel + 255) / 256, 256, 0, stream>>>(f, ps, n, firstPixel, endPixel); }
-    ctx->launches++;
-    GFX_CUDA(ctx, cudaGetLastError());
+    rc = launchWavefrontFrame(
+        ctx, stream, p, s, ps, numRounds,
+        WavefrontLabels{ "nrc_first_hit", "nrc_trace_shadow", "nrc_trace_extension", "nrc_bounce", "nrc_finish" },
+        NrcShadowWriter{ ps.shadowPixel, ps.shadowPending, n.shadowPending2, ps.radiance, n.stagedIndex, n.trainTarget[0] }, true,
+        [&](dim3 grid, dim3 block) {
+            if (bump)
+                k_nrcFirstHit<true><<<grid, block, 0, stream>>>(s, f, p, ps, n);
+            else
+                k_nrcFirstHit<false><<<grid, block, 0, stream>>>(s, f, p, ps, n);
+        },
+        [&](uint32_t blocks, uint32_t round) {
+            if (bump)
+                k_nrcBounce<true><<<blocks, 64, 0, stream>>>(s, f, p, ps, n, round);
+            else
+                k_nrcBounce<false><<<blocks, 64, 0, stream>>>(s, f, p, ps, n, round);
+        },
+        [&] {
+            GFX_TIMED(ctx, stream, "nrc_commit");
+            k_nrcCommitScan<<<1, 1024, 0, stream>>>(n, p.bufferIndex, F.W, F.H);
+            if (sharded) // one word per rank and round: the only exchange the path tracer needs
+                commitError |= allGather(n.shardCounts + 64, n.shardCounts, 1, 3 /* ncclUint32 */, F.nrc.shardComm, stream);
+            k_nrcCommitScatter<<<scatterGrid, 128, 0, stream>>>(n, numPixels, p.bufferIndex);
+            ctx->launches += 2;
+            if (sharded) {
+                k_nrcCommitAdvance<<<1, 1, 0, stream>>>(n, p.bufferIndex);
+                ctx->launches++;
+            }
+        },
+        [&](uint32_t blocks) {
+            const uint32_t firstPixel = p.y0 * F.W, endPixel = p.y1 * F.W;
+            k_nrcFinish<<<blocks, 256, 0, stream>>>(f, ps, n, firstPixel, endPixel);
+        });
+    if (rc != GFX_OK)
+        return rc;
     if (commitError) {
         ctx->setError("gfx_pathtrace_launch(GFX_PT_NRC): ncclAllGather of the training-vertex counts failed");
         return GFX_ERR_CUDA;
@@ -831,22 +781,18 @@ __global__ void __launch_bounds__(64) k_nrcVisualizeQueries(DevScene s, DevFrame
     const uint4 gb0 = f.gb0[p.bufferIndex][pix];
     const bool hit = gb0.x != 0xFFFFFFFFu;
     if (hit) {
-        const DevInstance* inst = s.instances + gb0.x;
-        const DevMesh mesh = s.meshes[gb0.y];
-        const float bcB = decodeBarycentric((uint16_t)(gb0.w & 0xFFFFu));
-        const float bcC = decodeBarycentric((uint16_t)(gb0.w >> 16));
-        SurfacePoint sp;
-        computeSurfacePointFromGBuffer(s, inst, mesh, gb0.z, bcB, bcC, &sp);
-        f3 vOut = p.camera.position - sp.positionInWorld;
+        GBufferHit h;
+        decodeGBufferHit(s, gb0, &h);
+        f3 vOut = p.camera.position - h.sp.positionInWorld;
         const float primaryDist2 = sqLength(vOut);
         vOut /= sqrtf(primaryDist2);
-        const float primaryDotVN = dot(vOut, sp.geometricNormalInWorld);
+        const float primaryDotVN = dot(vOut, h.sp.geometricNormalInWorld);
         const float frontHit = primaryDotVN >= 0.0f ? 1.0f : -1.0f;
-        const f3 positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
-        ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+        const f3 positionInWorld = offsetRayOrigin(h.sp.positionInWorld, frontHit * h.sp.geometricNormalInWorld);
+        ReferenceFrame shadingFrame(h.sp.shadingNormalInWorld, h.sp.texCoord0DirInWorld);
         if (BUMP) // :740-743
-            shadingFrame = bumpShadingFrameAtHit(s, mesh, gb0.z, bcB, bcC, shadingFrame);
-        const BSDF bsdf = setupBsdfAtHit(s, mesh, gb0.z, bcB, bcC);
+            shadingFrame = bumpShadingFrameAtHit(s, h.mesh, gb0.z, h.bcB, h.bcC, shadingFrame);
+        const BSDF bsdf = setupBsdfAtHit(s, h.mesh, gb0.z, h.bcB, h.bcC);
         createRadianceQuery(p, positionInWorld, shadingFrame.normal, vOut, bsdf, n.inferenceQuery + 14 * (size_t)pix);
     }
     n.terminalInfo[pix] = packTerminalInfo(f3(1.0f), 1, hit, false, false);

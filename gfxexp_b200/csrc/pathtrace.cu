@@ -60,6 +60,9 @@ GFX_D void shadeVertexVariant(const DevScene &s, const DevRegir &rg, const DevFr
     }
 }
 
+// the bounce kernel's variants: GFX_PT_BASELINE, GFX_PT_REGIR, and GFX_PT_SVGF without and with GFX_SVGF_MOLLIFY_SPECULAR
+enum class PtVariant { Baseline, Regir, Svgf, SvgfMollify };
+
 // pathTrace_rayGen_generic up to the path extension loop (:73-160).  BUMP: GfxFrameParams::enableBumpMapping (a kernel of its own,
 // so that the frames without it run the code they ran before it existed; likewise k_ptBounce)
 template <bool REGIR, bool BUMP>
@@ -78,28 +81,23 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptFirstHit(DevScene s, DevFrame f, DevFrameP
         const uint4 gb0 = f.gb0[p.bufferIndex][pix];
         f3 radiance(0.001f, 0.001f, 0.001f);
         if (gb0.x != 0xFFFFFFFFu) {
-            const DevInstance* inst = s.instances + gb0.x;
-            const DevMesh mesh = s.meshes[gb0.y];
-            const float bcB = decodeBarycentric((uint16_t)(gb0.w & 0xFFFFu));
-            const float bcC = decodeBarycentric((uint16_t)(gb0.w >> 16));
-            SurfacePoint sp;
-            computeSurfacePointFromGBuffer(s, inst, mesh, gb0.z, bcB, bcC, &sp);
-
+            GBufferHit h;
+            decodeGBufferHit(s, gb0, &h);
             const f3 alpha(1.0f);
             PCG32RNG rng{ f.rng[pix] };
-            const GfxMaterialDesc* mat = s.materials + mesh.materialSlot;
-            const f3 vOut = normalize(p.camera.position - sp.positionInWorld);
-            const float frontHit = dot(vOut, sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
-            positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
-            ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
+            const GfxMaterialDesc* mat = s.materials + h.mesh.materialSlot;
+            const f3 vOut = normalize(p.camera.position - h.sp.positionInWorld);
+            const float frontHit = dot(vOut, h.sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
+            positionInWorld = offsetRayOrigin(h.sp.positionInWorld, frontHit * h.sp.geometricNormalInWorld);
+            ReferenceFrame shadingFrame(h.sp.shadingNormalInWorld, h.sp.texCoord0DirInWorld);
             if (BUMP) // path_tracing :117-121, regir :200-203
-                shadingFrame = bumpShadingFrameAtHit(s, mesh, gb0.z, bcB, bcC, shadingFrame);
+                shadingFrame = bumpShadingFrameAtHit(s, h.mesh, gb0.z, h.bcB, h.bcC, shadingFrame);
             const f3 vOutLocal = shadingFrame.toLocal(vOut);
 
             radiance = f3(0.0f);
             if (vOutLocal.z > 0 && mat->hasEmittance)
                 radiance += alpha * f3(mat->emittance[0], mat->emittance[1], mat->emittance[2]) / kPi;
-            const BSDF bsdf = setupBsdfAtHit(s, mesh, gb0.z, bcB, bcC);
+            const BSDF bsdf = setupBsdfAtHit(s, h.mesh, gb0.z, h.bcB, h.bcC);
             shadeVertexVariant<REGIR>(s, rg, p, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, 1u, &radiance, &v);
             f.rng[pix] = rng.state;
             ps.alphaPdf[pix] = make_float4(v.alpha.x, v.alpha.y, v.alpha.z, v.dirPDensity);
@@ -114,10 +112,14 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptFirstHit(DevScene s, DevFrame f, DevFrameP
 }
 
 // pathTrace_closestHit_generic (:218-300) + the bookkeeping of the path extension loop (:161-194) for the
-// compacted queue of live paths; `round` = pathLength - 2 selects the queue parity and the counters.
-template <bool REGIR, bool BUMP>
+// compacted queue of live paths; `round` = pathLength - 2 selects the queue parity and the counters.  The SVGF app's
+// closest-hit program (svgf :381-468) and miss program (:482-513) are the baseline's but for two differences: no Russian
+// roulette at pathLength 2 (round 0), whose random number is still drawn (:438-441), and with SvgfMollify the BSDF set up with
+// BSDFFlags::Regularize (:446-450).
+template <PtVariant V, bool BUMP>
 __global__ void GFX_BOUNCE_BOUNDS k_ptBounce(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, DevRegir rg, uint32_t round,
-                                                 uint32_t maxLengthTerminate) {
+                                             uint32_t maxLengthTerminate) {
+    constexpr bool REGIR = V == PtVariant::Regir, SVGF = V == PtVariant::Svgf || V == PtVariant::SvgfMollify;
     const uint32_t curQueue = round & 1u, nextQueue = curQueue ^ 1u;
     const uint32_t* roundCounters = ps.counters + 4 * round;
     uint32_t* nextCounters = ps.counters + 4 * (round + 1);
@@ -148,39 +150,28 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptBounce(DevScene s, DevFrame f, DevFramePar
                 f3 radiance(rad.x, rad.y, rad.z);
                 PCG32RNG rng{ f.rng[pix] };
 
-                const uint2 im = __ldg(s.geomToInstMesh + hit.x);
-                const DevInstance* inst = s.instances + im.x;
-                const DevMesh mesh = s.meshes[im.y];
-                SurfacePoint sp;
-                computeSurfacePointAtHit(s, inst, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), &sp);
-                if (REGIR) // regir's closest-hit program never computes it (uninitialised in the reference): defined as 0
-                    sp.hypAreaPDensity = 0.0f;
-                const GfxMaterialDesc* mat = s.materials + mesh.materialSlot;
-
-                const f3 vOut = normalize(-rayDir);
-                const float frontHit = dot(vOut, sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
-                ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
-                if (BUMP) // path_tracing :252-255, regir :336-339
-                    shadingFrame = bumpShadingFrameAtHit(s, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), shadingFrame);
-                positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
-                const f3 vOutLocal = shadingFrame.toLocal(vOut);
+                HitVertex h;
+                setupHitVertex<BUMP>(s, hit, rayDir, &h);
+                positionInWorld = h.positionInWorld;
+                const GfxMaterialDesc* mat = s.materials + h.mesh.materialSlot;
 
                 // implicit light sampling, MIS against the hypothetical NEE density (:262-275)
-                if (vOutLocal.z > 0 && mat->hasEmittance) {
+                if (h.vOutLocal.z > 0 && mat->hasEmittance) {
                     const f3 emittance(mat->emittance[0], mat->emittance[1], mat->emittance[2]);
                     const float dist2 = sqLength(positionInWorld - rayOrigin);
-                    const float lightPDensity = sp.hypAreaPDensity * dist2 / vOutLocal.z;
-                    const float bsdfPDensity = prevDirPDensity;
-                    const float misWeight = pow2f(bsdfPDensity) / (pow2f(bsdfPDensity) + pow2f(lightPDensity));
-                    radiance += alpha * emittance * (misWeight / kPi);
+                    // regir's closest-hit program never computes the density (uninitialised in the reference): defined as 0
+                    const float hypAreaPDensity = REGIR ? 0.0f : h.sp.hypAreaPDensity;
+                    radiance += alpha * emittance * implicitEmissionWeight(hypAreaPDensity, dist2, h.vOutLocal.z, prevDirPDensity);
                 }
 
                 // Russian roulette (:277-281)
-                const float continueProb = fminf(sRGB_calcLuminance(alpha) / initImportance, 1.0f);
+                const float continueProb = SVGF && round == 0 ? 1.0f : fminf(sRGB_calcLuminance(alpha) / initImportance, 1.0f);
                 if (!(rng.getFloat0cTo1o() >= continueProb || maxLengthTerminate)) {
                     alpha /= continueProb;
-                    const BSDF bsdf = setupBsdfAtHit(s, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w));
-                    shadeVertexVariant<REGIR>(s, rg, p, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, round + 2, &radiance, &v);
+                    const BSDF bsdf = setupBsdfAtHit<V == PtVariant::SvgfMollify>(s, h.mesh, hit.y, __uint_as_float(hit.z),
+                                                                                  __uint_as_float(hit.w));
+                    shadeVertexVariant<REGIR>(s, rg, p, positionInWorld, h.vOutLocal, h.shadingFrame, bsdf, rng, alpha, round + 2,
+                                              &radiance, &v);
                     ps.alphaPdf[pix] = make_float4(v.alpha.x, v.alpha.y, v.alpha.z, v.dirPDensity);
                     alive = true;
                 }
@@ -188,14 +179,7 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptBounce(DevScene s, DevFrame f, DevFramePar
                 ps.radiance[pix] = make_float4(radiance.x, radiance.y, radiance.z, 0.0f);
             }
             else if (!REGIR && s.env.enabled) { // miss program (:310-341); the ReGIR ray type's miss program is empty
-                const uint32_t missPix = ps.extPixel[curQueue][slot];
-                const float4 r1 = ps.extRays[curQueue][2 * (size_t)slot + 1];
-                const float4 ap = ps.alphaPdf[missPix];
-                const f3 implicit = evaluateEnvLightOnMiss(s, f3(r1.x, r1.y, r1.z), ap.w, false);
-                float4 rad = ps.radiance[missPix];
-                const f3 add = f3(ap.x, ap.y, ap.z) * implicit;
-                rad.x += add.x; rad.y += add.y; rad.z += add.z;
-                ps.radiance[missPix] = rad;
+                addEnvLightOnMiss(s, ps, curQueue, slot, ps.extPixel[curQueue][slot], false);
             }
         }
         emitRays(s, ps, nextCounters, nextQueue, lane, pix, positionInWorld, v, alive);
@@ -260,6 +244,7 @@ DevPathState makePathState(const gfx_ctx* ctx) {
 // runs.  The first vertex is the raster G-buffer's: position, interpolated and normalised shading normal, texture
 // coordinate.  The geometric normal is that shading normal (:237), the frame is ReferenceFrame(normal) (no texture-coordinate
 // tangent) and the origin is offset naively (:242).  Miss pixels return at once (:213-219): no RNG draw, no environment.
+// The bounces are k_ptBounce<PtVariant::Svgf / SvgfMollify>.
 __global__ void GFX_BOUNCE_BOUNDS k_ptSvgfFirstHit(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps) {
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
     const uint32_t y = p.y0 + blockIdx.y * 8 + threadIdx.y;
@@ -276,26 +261,21 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptSvgfFirstHit(DevScene s, DevFrame f, DevFr
         f3 radiance(0.0f);
         float4 albedo = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         if (gb0.x != 0xFFFFFFFFu) {
-            const DevInstance* inst = s.instances + gb0.x;
-            const DevMesh mesh = s.meshes[gb0.y];
-            const float bcB = decodeBarycentric((uint16_t)(gb0.w & 0xFFFFu));
-            const float bcC = decodeBarycentric((uint16_t)(gb0.w >> 16));
-            SurfacePoint sp;
-            computeSurfacePointFromGBuffer(s, inst, mesh, gb0.z, bcB, bcC, &sp);
-
+            GBufferHit h;
+            decodeGBufferHit(s, gb0, &h);
             const f3 alpha(1.0f);
             PCG32RNG rng{ f.rng[pix] };
-            const GfxMaterialDesc* mat = s.materials + mesh.materialSlot;
-            const f3 shadingNormalInWorld = sp.shadingNormalInWorld;
-            const f3 vOut = normalize(p.camera.position - sp.positionInWorld);
+            const GfxMaterialDesc* mat = s.materials + h.mesh.materialSlot;
+            const f3 shadingNormalInWorld = h.sp.shadingNormalInWorld;
+            const f3 vOut = normalize(p.camera.position - h.sp.positionInWorld);
             const float frontHit = dot(vOut, shadingNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
             const ReferenceFrame shadingFrame(shadingNormalInWorld);
-            positionInWorld = offsetRayOriginNaive(sp.positionInWorld, frontHit * shadingNormalInWorld);
+            positionInWorld = offsetRayOriginNaive(h.sp.positionInWorld, frontHit * shadingNormalInWorld);
             const f3 vOutLocal = shadingFrame.toLocal(vOut);
 
             if (vOutLocal.z > 0 && mat->hasEmittance)
                 radiance += alpha * f3(mat->emittance[0], mat->emittance[1], mat->emittance[2]) / kPi;
-            const BSDF bsdf = setupBsdfAtHit(s, mesh, gb0.z, bcB, bcC);
+            const BSDF bsdf = setupBsdfAtHit(s, h.mesh, gb0.z, h.bcB, h.bcC);
             const f3 dhReflectance = bsdf.evaluateDHReflectanceEstimate(vOutLocal); // :256; the 0.001 threshold is the temporal pass's
             albedo = make_float4(dhReflectance.x, dhReflectance.y, dhReflectance.z, 1.0f);
             shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, &radiance, &v);
@@ -307,92 +287,6 @@ __global__ void GFX_BOUNCE_BOUNDS k_ptSvgfFirstHit(DevScene s, DevFrame f, DevFr
         f.albedo[pix] = albedo;
     }
     emitRays(s, ps, ps.counters, 0u, lane, pix, positionInWorld, v, alive);
-}
-
-// The SVGF app's closest-hit program (:381-468) and miss program (:482-513) on the compacted queue, as k_ptBounce without ReGIR:
-// no Russian roulette at pathLength 2 (round 0), whose random number is still drawn (:438-441), and with MOLLIFY the BSDF
-// set up with BSDFFlags::Regularize (:446-450).  A kernel of its own, so that k_ptBounce's code stays as it is.
-template <bool MOLLIFY>
-__global__ void GFX_BOUNCE_BOUNDS k_ptSvgfBounce(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, uint32_t round,
-                                                 uint32_t maxLengthTerminate) {
-    const uint32_t curQueue = round & 1u, nextQueue = curQueue ^ 1u;
-    const uint32_t* roundCounters = ps.counters + 4 * round;
-    uint32_t* nextCounters = ps.counters + 4 * (round + 1);
-    const uint32_t count = roundCounters[0];
-    const uint32_t lane = threadIdx.x & 31u;
-    const uint32_t warpsPerGrid = gridDim.x * (blockDim.x >> 5);
-    const uint32_t warp = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    const float initImportance = sRGB_calcLuminance(f3(1.0f));
-
-    for (uint32_t base = warp * 32u; base < count; base += warpsPerGrid * 32u) {
-        const uint32_t slot = base + lane;
-        bool alive = false;
-        uint32_t pix = 0;
-        f3 positionInWorld(0.0f);
-        VertexOutput v;
-        v.wantShadow = v.wantExtension = false;
-        if (slot < count) {
-            const uint4 hit = ps.extHits[slot];
-            if (hit.y != 0xFFFFFFFFu) { // miss program: no environment light, the path ends
-                pix = ps.extPixel[curQueue][slot];
-                const float4 r0 = ps.extRays[curQueue][2 * (size_t)slot];
-                const float4 r1 = ps.extRays[curQueue][2 * (size_t)slot + 1];
-                const f3 rayOrigin(r0.x, r0.y, r0.z), rayDir(r1.x, r1.y, r1.z);
-                const float4 ap = ps.alphaPdf[pix];
-                f3 alpha(ap.x, ap.y, ap.z);
-                const float prevDirPDensity = ap.w;
-                const float4 rad = ps.radiance[pix];
-                f3 radiance(rad.x, rad.y, rad.z);
-                PCG32RNG rng{ f.rng[pix] };
-
-                const uint2 im = __ldg(s.geomToInstMesh + hit.x);
-                const DevInstance* inst = s.instances + im.x;
-                const DevMesh mesh = s.meshes[im.y];
-                SurfacePoint sp;
-                computeSurfacePointAtHit(s, inst, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), &sp);
-                const GfxMaterialDesc* mat = s.materials + mesh.materialSlot;
-
-                const f3 vOut = normalize(-rayDir);
-                const float frontHit = dot(vOut, sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
-                const ReferenceFrame shadingFrame(sp.shadingNormalInWorld, sp.texCoord0DirInWorld);
-                positionInWorld = offsetRayOrigin(sp.positionInWorld, frontHit * sp.geometricNormalInWorld);
-                const f3 vOutLocal = shadingFrame.toLocal(vOut);
-
-                // implicit light sampling, MIS against the hypothetical NEE density (:422-435)
-                if (vOutLocal.z > 0 && mat->hasEmittance) {
-                    const f3 emittance(mat->emittance[0], mat->emittance[1], mat->emittance[2]);
-                    const float dist2 = sqLength(positionInWorld - rayOrigin);
-                    const float lightPDensity = sp.hypAreaPDensity * dist2 / vOutLocal.z;
-                    const float bsdfPDensity = prevDirPDensity;
-                    const float misWeight = pow2f(bsdfPDensity) / (pow2f(bsdfPDensity) + pow2f(lightPDensity));
-                    radiance += alpha * emittance * (misWeight / kPi);
-                }
-
-                // Russian roulette (:437-444)
-                const float continueProb = round == 0 ? 1.0f : fminf(sRGB_calcLuminance(alpha) / initImportance, 1.0f);
-                if (!(rng.getFloat0cTo1o() >= continueProb || maxLengthTerminate)) {
-                    alpha /= continueProb;
-                    const BSDF bsdf = setupBsdfAtHit<MOLLIFY>(s, mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w));
-                    shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, &radiance, &v);
-                    ps.alphaPdf[pix] = make_float4(v.alpha.x, v.alpha.y, v.alpha.z, v.dirPDensity);
-                    alive = true;
-                }
-                f.rng[pix] = rng.state;
-                ps.radiance[pix] = make_float4(radiance.x, radiance.y, radiance.z, 0.0f);
-            }
-            else if (s.env.enabled) { // miss program (:482-513)
-                const uint32_t missPix = ps.extPixel[curQueue][slot];
-                const float4 r1 = ps.extRays[curQueue][2 * (size_t)slot + 1];
-                const float4 ap = ps.alphaPdf[missPix];
-                const f3 implicit = evaluateEnvLightOnMiss(s, f3(r1.x, r1.y, r1.z), ap.w, false);
-                float4 rad = ps.radiance[missPix];
-                const f3 add = f3(ap.x, ap.y, ap.z) * implicit;
-                rad.x += add.x; rad.y += add.y; rad.z += add.z;
-                ps.radiance[missPix] = rad;
-            }
-        }
-        emitRays(s, ps, nextCounters, nextQueue, lane, pix, positionInWorld, v, alive);
-    }
 }
 
 // :318-319: contribution = max(contribution, RGB(0.0f)), component-wise std::fmax: a NaN component becomes 0.  The single-spp
@@ -407,50 +301,47 @@ __global__ void __launch_bounds__(256) k_ptSvgfEpilogue(DevFrame f, DevFramePara
     f.beauty[pix] = make_float4(rad.x > 0.0f ? rad.x : 0.0f, rad.y > 0.0f ? rad.y : 0.0f, rad.z > 0.0f ? rad.z : 0.0f, 1.0f);
 }
 
-static int launchPathTraceSvgf(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params) {
+template <PtVariant V, bool BUMP>
+static int launchPathTraceVariant(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params) {
+    constexpr bool REGIR = V == PtVariant::Regir, SVGF = V == PtVariant::Svgf || V == PtVariant::SvgfMollify;
     const int rc = ensurePathTraceBuffers(ctx);
     if (rc != GFX_OK)
         return rc;
-    FrameState &F = ctx->frame;
     DevFrameParams p = makeDevParams(ctx, params);
     if (p.y1 <= p.y0)
         return GFX_OK;
-    p.maxPathLength = params->maxPathLength ? params->maxPathLength : 5u; // svgf_main.cpp:1729
-    const bool mollify = (params->svgfFlags & GFX_SVGF_MOLLIFY_SPECULAR) != 0;
+    p.maxPathLength = params->maxPathLength ? params->maxPathLength : 5u; // 0 = the hosts' default (svgf_main.cpp:1729)
     const DevScene s = ctx->devScene(params);
     const DevFrame f = ctx->devFrame();
     const DevPathState ps = makePathState(ctx);
+    DevRegir rg = {};
+    if (REGIR)
+        rg = makeDevRegir(ctx, params);
 
     const uint32_t maxPathLength = p.maxPathLength;
     const uint32_t numRounds = min(max(maxPathLength, 2u) - 1u, kMaxPathRounds); // pathLength = 2 .. maxPathLength
-    GFX_CUDA(ctx, cudaMemsetAsync(F.ptCounters, 0, (kMaxPathRounds + 1) * 16, stream));
-
-    const dim3 block(8, 8);
-    const dim3 grid((F.W + 7) / 8, (p.y1 - p.y0 + 7) / 8);
-    { GFX_TIMED(ctx, stream, "pt_svgf_first_hit"); k_ptSvgfFirstHit<<<grid, block, 0, stream>>>(s, f, p, ps); }
-    ctx->launches++;
-    const int traceGrid = wavefrontGrid();
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
-    const ShadowAccumulateWriter shadowWriter{ ps.shadowPixel, ps.shadowPending, ps.radiance };
-    const ExtensionHitWriter extWriter{ ps.extHits };
-    for (uint32_t round = 0; round < numRounds; ++round) {
-        uint32_t* c = F.ptCounters + 4 * round;
-        { GFX_TIMED(ctx, stream, "pt_trace_shadow"); k_traceWavefront<true, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.shadowRays, c + 2, 0u, c + 3, shadowWriter); }
-        { GFX_TIMED(ctx, stream, "pt_trace_extension"); k_traceWavefront<false, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.extRays[round & 1], c + 0, 0u, c + 1, extWriter); }
-        const uint32_t maxLengthTerminate = (round + 2 >= maxPathLength || round + 1 == numRounds) ? 1u : 0u;
-        GFX_TIMED(ctx, stream, "pt_svgf_bounce");
-        if (mollify)
-            k_ptSvgfBounce<true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, round, maxLengthTerminate);
-        else
-            k_ptSvgfBounce<false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, round, maxLengthTerminate);
-        ctx->launches += 3;
-    }
-    const uint32_t numPixels = (p.y1 - p.y0) * F.W;
-    { GFX_TIMED(ctx, stream, "pt_svgf_epilogue"); k_ptSvgfEpilogue<<<(numPixels + 255) / 256, 256, 0, stream>>>(f, p, ps); }
-    ctx->launches++;
-    GFX_CUDA(ctx, cudaGetLastError());
-    return GFX_OK;
+    const WavefrontLabels labels = SVGF ? WavefrontLabels{ "pt_svgf_first_hit", "pt_trace_shadow", "pt_trace_extension", "pt_svgf_bounce", "pt_svgf_epilogue" }
+                                        : WavefrontLabels{ "pt_first_hit", "pt_trace_shadow", "pt_trace_extension", "pt_bounce", "pt_accumulate" };
+    // the last round requests no rays (maxLengthTerminate), nothing is left in flight
+    return launchWavefrontFrame(
+        ctx, stream, p, s, ps, numRounds, labels, ShadowAccumulateWriter{ ps.shadowPixel, ps.shadowPending, ps.radiance }, false,
+        [&](dim3 grid, dim3 block) {
+            if constexpr (SVGF)
+                k_ptSvgfFirstHit<<<grid, block, 0, stream>>>(s, f, p, ps);
+            else
+                k_ptFirstHit<REGIR, BUMP><<<grid, block, 0, stream>>>(s, f, p, ps, rg);
+        },
+        [&](uint32_t blocks, uint32_t round) {
+            const uint32_t maxLengthTerminate = (round + 2 >= maxPathLength || round + 1 == numRounds) ? 1u : 0u;
+            k_ptBounce<V, BUMP><<<blocks, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
+        },
+        [] {},
+        [&](uint32_t blocks) {
+            if constexpr (SVGF)
+                k_ptSvgfEpilogue<<<blocks, 256, 0, stream>>>(f, p, ps);
+            else
+                k_ptAccumulate<<<blocks, 256, 0, stream>>>(f, p, ps);
+        });
 }
 
 int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, int variant) {
@@ -463,76 +354,25 @@ int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* par
         return launchPathTraceNrc(ctx, stream, params);
     if (variant == GFX_PT_NRC_VISUALIZE_PREDICTION)
         return launchNrcVisualizePrediction(ctx, stream, params);
-    if (variant == GFX_PT_SVGF)
-        return launchPathTraceSvgf(ctx, stream, params);
+    if (variant == GFX_PT_SVGF) { // the SVGF app has no bump mapping
+        if (params->svgfFlags & GFX_SVGF_MOLLIFY_SPECULAR)
+            return launchPathTraceVariant<PtVariant::SvgfMollify, false>(ctx, stream, params);
+        return launchPathTraceVariant<PtVariant::Svgf, false>(ctx, stream, params);
+    }
     if (variant != GFX_PT_BASELINE && variant != GFX_PT_REGIR) {
         ctx->setError("gfx_pathtrace_launch: unknown variant");
         return GFX_ERR_INVALID_ARGUMENT;
     }
-    const bool regir = variant == GFX_PT_REGIR;
-    if (regir && !ctx->frame.regir.created) {
+    const bool bump = params->enableBumpMapping != 0;
+    if (variant == GFX_PT_BASELINE)
+        return bump ? launchPathTraceVariant<PtVariant::Baseline, true>(ctx, stream, params)
+                    : launchPathTraceVariant<PtVariant::Baseline, false>(ctx, stream, params);
+    if (!ctx->frame.regir.created) {
         ctx->setError("gfx_pathtrace_launch(GFX_PT_REGIR): call gfx_regir_build_cells first");
         return GFX_ERR_NOT_READY;
     }
-    const int rc = ensurePathTraceBuffers(ctx);
-    if (rc != GFX_OK)
-        return rc;
-    FrameState &F = ctx->frame;
-    DevFrameParams p = makeDevParams(ctx, params);
-    if (p.y1 <= p.y0)
-        return GFX_OK;
-    p.maxPathLength = params->maxPathLength ? params->maxPathLength : 5u; // 0 = the hosts' default
-    const DevScene s = ctx->devScene(params);
-    const DevFrame f = ctx->devFrame();
-    const DevPathState ps = makePathState(ctx);
-    DevRegir rg = {};
-    if (regir)
-        rg = makeDevRegir(ctx, params);
-
-    const uint32_t maxPathLength = p.maxPathLength;
-    const uint32_t numRounds = min(max(maxPathLength, 2u) - 1u, kMaxPathRounds); // pathLength = 2 .. maxPathLength
-    GFX_CUDA(ctx, cudaMemsetAsync(F.ptCounters, 0, (kMaxPathRounds + 1) * 16, stream));
-
-    const dim3 block(8, 8);
-    const dim3 grid((F.W + 7) / 8, (p.y1 - p.y0 + 7) / 8);
-    const bool bump = params->enableBumpMapping != 0;
-    { GFX_TIMED(ctx, stream, "pt_first_hit");
-    if (regir && bump)
-        k_ptFirstHit<true, true><<<grid, block, 0, stream>>>(s, f, p, ps, rg);
-    else if (regir)
-        k_ptFirstHit<true, false><<<grid, block, 0, stream>>>(s, f, p, ps, rg);
-    else if (bump)
-        k_ptFirstHit<false, true><<<grid, block, 0, stream>>>(s, f, p, ps, rg);
-    else
-        k_ptFirstHit<false, false><<<grid, block, 0, stream>>>(s, f, p, ps, rg); }
-    ctx->launches++;
-    const int traceGrid = wavefrontGrid();
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
-    const ShadowAccumulateWriter shadowWriter{ ps.shadowPixel, ps.shadowPending, ps.radiance };
-    const ExtensionHitWriter extWriter{ ps.extHits };
-    for (uint32_t round = 0; round < numRounds; ++round) {
-        uint32_t* c = F.ptCounters + 4 * round;
-        { GFX_TIMED(ctx, stream, "pt_trace_shadow"); k_traceWavefront<true, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.shadowRays, c + 2, 0u, c + 3, shadowWriter); }
-        { GFX_TIMED(ctx, stream, "pt_trace_extension"); k_traceWavefront<false, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.extRays[round & 1], c + 0, 0u, c + 1, extWriter); }
-        const uint32_t maxLengthTerminate = (round + 2 >= maxPathLength || round + 1 == numRounds) ? 1u : 0u;
-        GFX_TIMED(ctx, stream, "pt_bounce");
-        if (regir && bump)
-            k_ptBounce<true, true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
-        else if (regir)
-            k_ptBounce<true, false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
-        else if (bump)
-            k_ptBounce<false, true><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
-        else
-            k_ptBounce<false, false><<<sms * 16, 64, 0, stream>>>(s, f, p, ps, rg, round, maxLengthTerminate);
-        ctx->launches += 3;
-    }
-    // the last round requests no rays (maxLengthTerminate), nothing is left in flight
-    const uint32_t numPixels = (p.y1 - p.y0) * F.W;
-    { GFX_TIMED(ctx, stream, "pt_accumulate"); k_ptAccumulate<<<(numPixels + 255) / 256, 256, 0, stream>>>(f, p, ps); }
-    ctx->launches++;
-    GFX_CUDA(ctx, cudaGetLastError());
-    return GFX_OK;
+    return bump ? launchPathTraceVariant<PtVariant::Regir, true>(ctx, stream, params)
+                : launchPathTraceVariant<PtVariant::Regir, false>(ctx, stream, params);
 }
 
 } // namespace gfx

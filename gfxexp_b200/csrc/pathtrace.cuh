@@ -188,6 +188,68 @@ GFX_D void computeSurfacePointAtHit(const DevScene &s, const DevInstance* inst, 
     sp->hypAreaPDensity = lightProb / area;
 }
 
+// the first hit as G-buffer 0 holds it (instance, mesh, triangle gb0.z, quantised barycentrics): mesh, barycentrics, surface point
+struct GBufferHit {
+    DevMesh mesh;
+    float bcB, bcC;
+    SurfacePoint sp;
+};
+GFX_D void decodeGBufferHit(const DevScene &s, const uint4 &gb0, GBufferHit* h) {
+    const DevInstance* inst = s.instances + gb0.x;
+    h->mesh = s.meshes[gb0.y];
+    h->bcB = decodeBarycentric((uint16_t)(gb0.w & 0xFFFFu));
+    h->bcC = decodeBarycentric((uint16_t)(gb0.w >> 16));
+    computeSurfacePointFromGBuffer(s, inst, h->mesh, gb0.z, h->bcB, h->bcC, &h->sp);
+}
+
+// the path vertex at an extension ray's hit (the closest-hit programs up to emission): the surface point, the ray origin of the
+// next rays offset to the side the ray arrived from (frontHit), the shading frame, bump-mapped with BUMP (path_tracing :252-255,
+// regir :336-339, neural_radiance_caching :398-401), and the outgoing direction in it
+struct HitVertex {
+    DevMesh mesh;
+    SurfacePoint sp;
+    f3 vOut, positionInWorld, vOutLocal;
+    ReferenceFrame shadingFrame;
+};
+template <bool BUMP>
+GFX_D void setupHitVertex(const DevScene &s, const uint4 &hit, const f3 &rayDir, HitVertex* h) {
+    const uint2 im = __ldg(s.geomToInstMesh + hit.x);
+    const DevInstance* inst = s.instances + im.x;
+    h->mesh = s.meshes[im.y];
+    computeSurfacePointAtHit(s, inst, h->mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), &h->sp);
+    h->vOut = normalize(-rayDir);
+    const float frontHit = dot(h->vOut, h->sp.geometricNormalInWorld) >= 0.0f ? 1.0f : -1.0f;
+    h->shadingFrame = ReferenceFrame(h->sp.shadingNormalInWorld, h->sp.texCoord0DirInWorld);
+    if (BUMP)
+        h->shadingFrame = bumpShadingFrameAtHit(s, h->mesh, hit.y, __uint_as_float(hit.z), __uint_as_float(hit.w), h->shadingFrame);
+    h->positionInWorld = offsetRayOrigin(h->sp.positionInWorld, frontHit * h->sp.geometricNormalInWorld);
+    h->vOutLocal = h->shadingFrame.toLocal(h->vOut);
+}
+
+// implicit light sampling at an emitter hit (path_tracing :262-275): the MIS weight against the hypothetical NEE density of the
+// point, over pi.  Each caller multiplies in the emittance and the path throughput in its reference's order, which rounds
+// differently: alpha * emittance * w (path_tracing, regir, svgf) or alpha * (emittance * w) (neural_radiance_caching).
+GFX_D float implicitEmissionWeight(float hypAreaPDensity, float dist2, float vOutLocalZ, float prevDirPDensity) {
+    const float lightPDensity = hypAreaPDensity * dist2 / vOutLocalZ;
+    const float bsdfPDensity = prevDirPDensity;
+    const float misWeight = pow2f(bsdfPDensity) / (pow2f(bsdfPDensity) + pow2f(lightPDensity));
+    return misWeight / kPi;
+}
+
+// the miss program of the bounce kernels (path_tracing :310-341): the environment along the extension ray of queue slot `slot`,
+// MIS-weighted against its NEE density, added to the radiance of pixel `pix` times the path throughput; returns the term
+// without the throughput (NRC adds it to its training target too)
+GFX_D f3 addEnvLightOnMiss(const DevScene &s, const DevPathState &ps, uint32_t queue, uint32_t slot, uint32_t pix, bool nrcVariant) {
+    const float4 r1 = ps.extRays[queue][2 * (size_t)slot + 1];
+    const float4 ap = ps.alphaPdf[pix];
+    const f3 implicit = evaluateEnvLightOnMiss(s, f3(r1.x, r1.y, r1.z), ap.w, nrcVariant);
+    float4 rad = ps.radiance[pix];
+    const f3 add = f3(ap.x, ap.y, ap.z) * implicit;
+    rad.x += add.x; rad.y += add.y; rad.z += add.z;
+    ps.radiance[pix] = rad;
+    return implicit;
+}
+
 // one slot of a compacted queue per requesting lane; one atomic per warp
 GFX_D uint32_t allocQueueSlot(uint32_t* counter, bool want, uint32_t lane) {
     const uint32_t mask = __ballot_sync(0xFFFFFFFFu, want);
@@ -400,8 +462,18 @@ GFX_D void neeRegir(const DevScene &s, const DevRegir &rg, const f3 &positionInW
     }
 }
 
+struct NoRayExtras {
+    template <class... A>
+    GFX_D void operator()(A...) const {}
+};
+
+// queues the rays a vertex requested.  A variant that keeps more per vertex passes onShadow(shadowSlot), run where the shadow
+// ray is written, and onQueued(), run once both rays are (NRC: emitRaysNrc).  The hooks are taken by reference: taken by value,
+// they made ptxas spill 10 more bytes in k_nrcBounce<true>.
+template <class OnShadow = NoRayExtras, class OnQueued = NoRayExtras>
 GFX_D void emitRays(const DevScene &s, const DevPathState &ps, uint32_t* roundCounters, uint32_t nextQueue, uint32_t lane,
-                    uint32_t pix, const f3 &positionInWorld, const VertexOutput &v, bool alive) {
+                    uint32_t pix, const f3 &positionInWorld, const VertexOutput &v, bool alive, const OnShadow &onShadow = {},
+                    const OnQueued &onQueued = {}) {
     const bool wantShadow = alive && v.wantShadow;
     const bool wantExt = alive && v.wantExtension;
     const uint32_t shadowSlot = allocQueueSlot(roundCounters + 2, wantShadow, lane);
@@ -411,12 +483,14 @@ GFX_D void emitRays(const DevScene &s, const DevPathState &ps, uint32_t* roundCo
         ps.shadowRays[2 * (size_t)shadowSlot + 1] = make_float4(v.shadowDir.x, v.shadowDir.y, v.shadowDir.z, v.shadowTmax);
         ps.shadowPixel[shadowSlot] = pix;
         ps.shadowPending[shadowSlot] = v.pending;
+        onShadow(shadowSlot);
     }
     if (wantExt) {
         ps.extRays[nextQueue][2 * (size_t)extSlot] = make_float4(positionInWorld.x, positionInWorld.y, positionInWorld.z, 0.0f);
         ps.extRays[nextQueue][2 * (size_t)extSlot + 1] = make_float4(v.nextDir.x, v.nextDir.y, v.nextDir.z, 3.402823466e+38f);
         ps.extPixel[nextQueue][extSlot] = pix;
     }
+    onQueued();
     // ray statistics (frame.stats[0]): one atomic per warp
     const uint32_t n = __popc(__ballot_sync(0xFFFFFFFFu, wantShadow)) + __popc(__ballot_sync(0xFFFFFFFFu, wantExt));
     if (lane == 0 && n)
@@ -455,5 +529,50 @@ struct ShadowAccumulateWriter { // visibility * (alpha * f * Le * G * misWeight 
         *dst = r;
     }
 };
+
+// ---- the host side of a frame ---------------------------------------------------------------------------------------------
+// the GFX_TIMED labels of a variant's launches: bench.py reports per-kernel times under them
+struct WavefrontLabels {
+    const char *firstHit, *traceShadow, *traceExtension, *bounce, *epilogue;
+};
+
+// One frame of a wavefront path tracer on the rows p.y0 .. p.y1 - 1, after the variant has checked its arguments and made
+// the frame's buffers: firstHit(grid, block) on 8x8-pixel blocks; then per round (pathLength = round + 2) the shadow rays and
+// the extension rays the previous vertex queued, traced by the persistent kernel, and bounce(blocks, round) on the compacted
+// queue of live paths, 16 blocks per SM; then epilogue(blocks) over the rows' pixels, 256 threads per block.  commit() runs
+// after the first-hit and every bounce launch (NRC numbers the training vertices staged there); with finalShadowTrace the
+// shadow rays of the last round are traced too (NRC's training paths sample a light there; the other variants request none).
+template <class ShadowWriter, class FirstHit, class Bounce, class Commit, class Epilogue>
+int launchWavefrontFrame(gfx_ctx* ctx, cudaStream_t stream, const DevFrameParams &p, const DevScene &s, const DevPathState &ps,
+                         uint32_t numRounds, const WavefrontLabels &labels, const ShadowWriter &shadowWriter,
+                         bool finalShadowTrace, FirstHit firstHit, Bounce bounce, Commit commit, Epilogue epilogue) {
+    GFX_CUDA(ctx, cudaMemsetAsync(ps.counters, 0, (kMaxPathRounds + 1) * 16, stream));
+    const uint32_t W = ctx->frame.W;
+    { GFX_TIMED(ctx, stream, labels.firstHit); firstHit(dim3((W + 7) / 8, (p.y1 - p.y0 + 7) / 8), dim3(8, 8)); }
+    commit();
+    ctx->launches++;
+    const int traceGrid = wavefrontGrid();
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, ctx->device);
+    const ExtensionHitWriter extWriter{ ps.extHits };
+    for (uint32_t round = 0; round < numRounds; ++round) {
+        uint32_t* c = ps.counters + 4 * round;
+        { GFX_TIMED(ctx, stream, labels.traceShadow); k_traceWavefront<true, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.shadowRays, c + 2, 0u, c + 3, shadowWriter); }
+        { GFX_TIMED(ctx, stream, labels.traceExtension); k_traceWavefront<false, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.extRays[round & 1], c + 0, 0u, c + 1, extWriter); }
+        { GFX_TIMED(ctx, stream, labels.bounce); bounce(sms * 16, round); }
+        commit();
+        ctx->launches += 3;
+    }
+    if (finalShadowTrace) {
+        uint32_t* c = ps.counters + 4 * numRounds;
+        k_traceWavefront<true, false><<<traceGrid, 128, 0, stream>>>(s.bvh, ps.shadowRays, c + 2, 0u, c + 3, shadowWriter);
+        ctx->launches++;
+    }
+    const uint32_t numPixels = (p.y1 - p.y0) * W;
+    { GFX_TIMED(ctx, stream, labels.epilogue); epilogue((numPixels + 255) / 256); }
+    ctx->launches++;
+    GFX_CUDA(ctx, cudaGetLastError());
+    return GFX_OK;
+}
 
 } // namespace gfx
