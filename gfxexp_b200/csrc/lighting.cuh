@@ -1,9 +1,10 @@
 // lighting.cuh — light sampling and direct-lighting helpers shared by the ReSTIR, ReGIR and path-tracing kernels.
 //
 // sampleLight<false> (restir_di/restir_di_shared.h:320-516; identical copies live in path_tracing_shared.h:220-482,
-// regir_shared.h, neural_radiance_caching_shared.h, svgf_shared.h), performDirectLighting (:518-557),
-// evaluateVisibility (:559-582).  Visibility rays run through the inline any-hit traversal of traverse.cuh
-// (fused kernels) or are queued for trace.cu's persistent kernel (wavefront kernels).
+// regir_shared.h, neural_radiance_caching_shared.h, svgf_shared.h), performDirectLighting (:518-557).  Visibility rays
+// run through the inline any-hit traversal of traverse.cuh (performDirectLighting<true>: ReSTIR's unbiased spatial pass)
+// or are queued for trace.cu's persistent kernel (evaluateVisibility :559-582 and the other ReSTIR passes' rays:
+// restir_common.cuh's visibilityRay; the wavefront path tracers' shadow rays).
 #pragma once
 #include "traverse.cuh"
 #include "shading.cuh"
@@ -143,21 +144,7 @@ GFX_D F8 pickGuideFetch(const DevScene &s, float ul) { // the guide entry of ul'
 }
 GFX_D LightPick pickLightFromGuide(const DevScene &s, float ul, const F8 &g);
 GFX_D LightPick pickLight(const DevScene &s, float ul) {
-#ifndef GFX_AB_CHAIN_PICK
     return pickLightFromGuide(s, ul, pickGuideFetch(s, ul));
-#else
-    LightPick r;
-    // A/B (-DGFX_AB_CHAIN_PICK): the definition instead of its flattened form
-    float unusedProb;
-    r.key = chainPickLightTriangle(s, ul, &unusedProb);
-    if (!(r.key & kPickNone)) {
-        const F8 h0 = ldg256(s.lightTris + kLightTriStride * (size_t)r.key);
-        r.sphere = h0.lo;
-        r.density = h0.hi.x;
-        r.instSlot = __float_as_uint(h0.hi.y);
-    }
-    return r;
-#endif
 }
 GFX_D LightPick pickLightFromGuide(const DevScene &s, float ul, const F8 &g) {
     LightPick r;
@@ -413,12 +400,7 @@ GFX_D bool sampleLightUnlessDark(const DevScene &s, float ul, float u0, float u1
         const float r = pick.sphere.w;
         const float t = -(dot(dc, shadingNormal) * vOutLocalZ);          // > 0: centre on the far side of the surface
         const float margin = t - 1.001f * r * fabsf(vOutLocalZ);
-#ifdef GFX_AB_NO_SPHERE
-        const bool sphereCull = false;
-#else
-        const bool sphereCull = true;
-#endif
-        if (sphereCull && r >= 0.0f && margin > 0.0f && margin * margin > 8e-6f * (sqLength(dc) + r * r) * (vOutLocalZ * vOutLocalZ)) {
+        if (r >= 0.0f && margin > 0.0f && margin * margin > 8e-6f * (sqLength(dc) + r * r) * (vOutLocalZ * vOutLocalZ)) {
             *areaPDensity = 1.0f; // any positive number: the caller only asks whether the density is positive
             return true;
         }
@@ -520,16 +502,6 @@ GFX_D bool traceVisibility(const DevScene &s, const f3 &org, const f3 &dir, floa
         atomicAdd(s.rayCounter, (unsigned long long)__popc(active));
     const Hit h = traverseBvh<true>(s.bvh, org, dir, 0.0f, tmax);
     return h.storageIndex == 0xFFFFFFFFu;
-}
-
-GFX_D bool evaluateVisibility(const DevScene &s, const f3 &shadingPoint, const LightSample &ls) { // :559-582
-    f3 shadowRayDir = ls.atInfinity ? ls.position : (ls.position - shadingPoint);
-    const float dist2 = sqLength(shadowRayDir);
-    float dist = sqrtf(dist2);
-    shadowRayDir /= dist;
-    if (ls.atInfinity)
-        dist = 1e+10f;
-    return traceVisibility(s, shadingPoint, shadowRayDir, dist * 0.9999f);
 }
 
 template <bool withVisibility>

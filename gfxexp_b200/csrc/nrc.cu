@@ -1679,12 +1679,11 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const uint32_t numTiles = numData / kTileRows; // upper bound when numDataPtr is given
-    // GFX_NRC_INFER_FUSED=1: the hash grid's one-kernel form (encode by L2 gathers inside the MLP kernel), the A/B arm; for both
-    // encodings it is also the path for buffers the TMA bulk copies cannot take (not 16-byte aligned)
+    // buffers the TMA bulk copies cannot take (not 16-byte aligned) go through the one-kernel form, which encodes by L2 gathers
+    // inside the MLP kernel
     const bool hashGrid = n->positionEncoding == GFX_NRC_POSITION_ENCODING_HASH_GRID;
-    const char* fusedEnv = getenv("GFX_NRC_INFER_FUSED");
     const bool aligned = (reinterpret_cast<uintptr_t>(inputData) & 15u) == 0 && (reinterpret_cast<uintptr_t>(predictionData) & 15u) == 0;
-    if ((hashGrid && fusedEnv && fusedEnv[0] == '1') || !aligned) {
+    if (!aligned) {
         const size_t smem = nrcInferFusedSmem(n->numMatrixWeights);
         auto kernel = hashGrid ? k_nrcInfer<kEncHashGrid> : k_nrcInfer<kEncTriangleWave>;
         NRC_CUDA(n, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

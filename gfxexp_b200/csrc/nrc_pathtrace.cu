@@ -16,13 +16,6 @@
 // neural_radiance_caching_main.cpp:2291-2304; here the inference launch reads its size from device memory).
 #include "pathtrace.cuh"
 
-// occupancy of the first-hit / bounce kernels: 16 blocks of 64 threads per SM = 64 registers, against the 88-128 ptxas picks
-// unconstrained (A/B: -DGFX_BOUNCE_MIN_BLOCKS=...)
-#ifndef GFX_BOUNCE_MIN_BLOCKS
-#define GFX_BOUNCE_MIN_BLOCKS 16
-#endif
-#define GFX_BOUNCE_BOUNDS __launch_bounds__(64, GFX_BOUNCE_MIN_BLOCKS)
-
 namespace gfx {
 
 constexpr float kPathTerminationFactor = 0.01f;        // neural_radiance_caching_shared.h:7

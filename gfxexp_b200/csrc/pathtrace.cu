@@ -22,13 +22,6 @@
 // float4 planes indexed by pixel.  The RNG draw order of every pixel is the reference's.
 #include "pathtrace.cuh"
 
-// occupancy of the first-hit / bounce kernels: 16 blocks of 64 threads per SM = 64 registers, against the 88-128 ptxas picks
-// unconstrained (A/B: -DGFX_BOUNCE_MIN_BLOCKS=...)
-#ifndef GFX_BOUNCE_MIN_BLOCKS
-#define GFX_BOUNCE_MIN_BLOCKS 16
-#endif
-#define GFX_BOUNCE_BOUNDS __launch_bounds__(64, GFX_BOUNCE_MIN_BLOCKS)
-
 namespace gfx {
 
 // One path vertex: NEE + next direction.  The ReGIR variant (regir/gpu_kernels/optix_pathtracing_kernels.cu) draws its

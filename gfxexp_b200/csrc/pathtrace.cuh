@@ -12,6 +12,10 @@ namespace gfx {
 
 constexpr uint32_t kMaxPathRounds = 64;
 
+// occupancy of the first-hit / bounce kernels: 16 blocks of 64 threads per SM = 64 registers, against the 88-128 ptxas picks
+// unconstrained
+#define GFX_BOUNCE_BOUNDS __launch_bounds__(64, 16)
+
 struct DevPathState {
     float4* alphaPdf;      // per pixel: alpha.rgb, prevDirPDensity
     float4* radiance;      // per pixel: contribution.rgb

@@ -5,8 +5,8 @@
 // Unbiased} / shading (restir_di/gpu_kernels/optix_restir_di_kernels.cu:14-287, 303-547, 559-637;
 // launch sites restir_di/restir_di_main.cpp:2378-2421) and the helpers they share
 // (sampleLight<false> restir_di_shared.h:320-516, performDirectLighting :518-557,
-// evaluateVisibility :559-582, testNeighbor :747-771).  Visibility rays run through the inline
-// any-hit traversal of traverse.cuh instead of optixTrace + the AH program.
+// evaluateVisibility :559-582, testNeighbor :747-771).  Visibility rays are queued for trace.cu's persistent any-hit
+// kernel instead of optixTrace + the AH program; the unbiased spatial pass traces its own inline (traverse.cuh).
 //
 // Per-pixel state is SoA: reservoirs are three float4 planes (Le|sumW, pos|M, n|-) so a pixel's own
 // reservoir is three coalesced 16-byte loads; neighbour gathers hit the same planes through L2.
@@ -15,13 +15,13 @@
 
 namespace gfx {
 
-// PHASE 0: the whole program in one kernel, visibility traced inline (megakernel form of the reference).
+// PHASE 0: the whole program in one kernel, for reuseVisibility = 0 (no visibility ray).
 // PHASE 1: candidates + recPDF, the visibility ray is only *requested* (wavefront form).
 // PHASE 2: applies the answered visibility, then the temporal merge.
 //
-// PHASE 1 runs the candidate loop in two phases (TWO_PHASE).  In a lock-step loop most candidates are dark and leave after the
-// staged light fetch, so everything after the bounding-sphere test - most of the kernel's issue slots - runs with a minority
-// of the 32 lanes.  Phase A walks all 2^n candidates in lock step but only draws ul,
+// PHASE 1 without an environment light runs the candidate loop in two phases.  In a lock-step loop most candidates are
+// dark and leave after the staged light fetch, so everything after the bounding-sphere test - most of the kernel's issue
+// slots - runs with a minority of the 32 lanes.  Phase A walks all 2^n candidates in lock step but only draws ul,
 // picks the light and tests its bounding sphere (the other three draws of a candidate are skipped with the LCG's 4-step
 // jump), leaving per lane a bit mask of survivors and their keys in shared memory.  Phase B is a per-lane loop over the
 // lane's own survivors, in candidate order: the PCG32 state at the candidate is rebuilt from the jump table, u0 / u1 / u
@@ -29,9 +29,9 @@ namespace gfx {
 // lock-step loop.  A warp then iterates max-over-lanes(#survivors) ~ 20 times instead of 32, with the expensive part at
 // a much higher lane utilisation; each pixel still sees the reference's sequence of Reservoir::update calls
 // (restir_di_shared.h:118-125) and draws, so results are bit-identical.
-constexpr uint32_t kRisMaxCandidates = 32; // TWO_PHASE keeps one key per candidate and thread in shared memory
+constexpr uint32_t kRisMaxCandidates = 32; // the two-phase loop keeps one key per candidate and thread in shared memory
 
-template <bool withTemporalRIS, bool useUnbiasedEstimator, int PHASE, bool TWO_PHASE, bool ENV>
+template <bool withTemporalRIS, bool useUnbiasedEstimator, int PHASE, bool ENV>
 GFX_D bool risPixel(const DevScene &s, const DevFrame &f, const DevFrameParams &p, RayRequest* request, uint32_t* candidateKeys) {
     // optix_restir_di_kernels.cu:14-287
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
@@ -80,7 +80,7 @@ GFX_D bool risPixel(const DevScene &s, const DevFrame &f, const DevFrameParams &
     bool hasSelection = false;
     bool selEnv = false; // ENV: the selected candidate came from the environment map
     float sumWeights = 0.0f;
-    if (TWO_PHASE && numCandidates <= kRisMaxCandidates) {
+    if (PHASE == 1 && !ENV && numCandidates <= kRisMaxCandidates) {
         uint32_t* myKeys = candidateKeys + (threadIdx.x + threadIdx.y * blockDim.x); // [candidate][64 threads]
         const uint64_t state0 = rng.state;
         // ---- phase A: ul, light pick, bounding sphere
@@ -210,7 +210,7 @@ GFX_D bool risPixel(const DevScene &s, const DevFrame &f, const DevFrameParams &
         selectedTargetDensity = info.y;
     }
 
-    if (p.reuseVisibility && selectedTargetDensity > 0.0f) {
+    if (PHASE != 0 && p.reuseVisibility && selectedTargetDensity > 0.0f) { // PHASE 0 runs only with reuseVisibility = 0
         if (PHASE == 1) {
             visibilityRay(positionInWorld, reservoir.sample, (uint32_t)pix, request);
             f.rng[pix] = rng.state;
@@ -218,8 +218,7 @@ GFX_D bool risPixel(const DevScene &s, const DevFrame &f, const DevFrameParams &
             f.reservoirInfo[curResIndex][pix] = make_float2(recPDFEstimate, selectedTargetDensity);
             return true;
         }
-        const bool visible = PHASE == 2 ? (f.visibility[pix] != 0) : evaluateVisibility(s, positionInWorld, reservoir.sample);
-        if (!visible) {
+        if (!f.visibility[pix]) {
             recPDFEstimate = 0.0f;
             selectedTargetDensity = 0.0f;
         }
@@ -314,22 +313,18 @@ GFX_D bool risPixel(const DevScene &s, const DevFrame &f, const DevFrameParams &
     return false;
 }
 
-#ifndef GFX_RIS_MIN_BLOCKS
 // 80 registers (8 B of spills): on an H100 80GB HBM3 at a 700 W power limit the 1080p two-phase candidate pass of bench.py
-// takes 1.93 ms at 12 blocks / SM against 2.24 ms at 16 (64 registers, 136 B of spills) (A/B: -DGFX_RIS_MIN_BLOCKS=...)
-#define GFX_RIS_MIN_BLOCKS 12
-#endif
-template <bool withTemporalRIS, bool useUnbiasedEstimator, int PHASE, bool TWO_PHASE = false, bool ENV = false>
-__global__ void __launch_bounds__(64, GFX_RIS_MIN_BLOCKS) k_initialAndTemporalRIS(DevScene s, DevFrame f, DevFrameParams p) {
-    static_assert(!TWO_PHASE || PHASE == 1, "the two-phase candidate loop belongs to the wavefront candidate pass");
-    static_assert(!(TWO_PHASE && ENV), "environment-light candidates go through the lock-step loop");
+// takes 1.93 ms at 12 blocks / SM against 2.24 ms at 16 (64 registers, 136 B of spills)
+constexpr int kRisMinBlocks = 12;
+template <bool withTemporalRIS, bool useUnbiasedEstimator, int PHASE, bool ENV = false>
+__global__ void __launch_bounds__(64, kRisMinBlocks) k_initialAndTemporalRIS(DevScene s, DevFrame f, DevFrameParams p) {
     RayRequest request;
     uint32_t* candidateKeys = nullptr;
-    if constexpr (TWO_PHASE) {
+    if constexpr (PHASE == 1 && !ENV) { // the two-phase candidate loop
         __shared__ uint32_t keys[kRisMaxCandidates * 64]; // [candidate][thread of the 8x8 block]
         candidateKeys = keys;
     }
-    const bool want = risPixel<withTemporalRIS, useUnbiasedEstimator, PHASE, TWO_PHASE, ENV>(s, f, p, &request, candidateKeys);
+    const bool want = risPixel<withTemporalRIS, useUnbiasedEstimator, PHASE, ENV>(s, f, p, &request, candidateKeys);
     if (PHASE == 1)
         enqueueRay(f, s.rayCounter, want, request);
 }
@@ -527,7 +522,6 @@ __global__ void __launch_bounds__(64) k_shadingRays(DevScene s, DevFrame f, DevF
     enqueueRay(f, s.rayCounter, want, request);
 }
 
-template <bool QUEUED_VISIBILITY>
 __global__ void __launch_bounds__(64) k_shading(DevScene s, DevFrame f, DevFrameParams p) {
     // optix_restir_di_kernels.cu:559-637
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
@@ -573,11 +567,9 @@ __global__ void __launch_bounds__(64) k_shading(DevScene s, DevFrame f, DevFrame
                 (!p.enableTemporalReuse || (p.enableSpatialReuse && p.useUnbiasedEstimator));
             if (visDone)
                 directCont = performDirectLighting<false>(s, positionInWorld, vOutLocal, shadingFrame, bsdf, lightSample);
-            else if (QUEUED_VISIBILITY) // performDirectLighting<true> with the answer of the wavefront trace
+            else // performDirectLighting<true> with the answer of the wavefront trace
                 directCont = f.visibility[pix] ? performDirectLighting<false>(s, positionInWorld, vOutLocal, shadingFrame, bsdf, lightSample)
                                                : f3(0.0f);
-            else
-                directCont = performDirectLighting<true>(s, positionInWorld, vOutLocal, shadingFrame, bsdf, lightSample);
         }
         contribution += recPDFEstimate * directCont;
     }
@@ -606,24 +598,18 @@ int launchReSTIR(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params
     const dim3 grid((ctx->frame.W + 7) / 8, (p.y1 - p.y0 + 7) / 8);
     const DevScene s = ctx->devScene(params);
     const DevFrame f = ctx->devFrame();
-    // wavefront form (default): request rays -> persistent-thread trace -> resolve.  GFX_MEGAKERNEL=1 selects
-    // the single-kernel form with inline traversal (same results; kept for A/B measurements).
-    static const bool megakernel = getenv("GFX_MEGAKERNEL") != nullptr;
-    const bool wave = !megakernel;
-    // the two-phase candidate loop (see risPixel) is the default; GFX_RIS_TWO_PHASE=0 selects the lock-step loop (A/B)
-    static const bool twoPhase = !(getenv("GFX_RIS_TWO_PHASE") && getenv("GFX_RIS_TWO_PHASE")[0] == '0');
+    // reuseVisibility: request rays -> persistent-thread trace -> resolve; otherwise the whole pass in one kernel
 #define RIS_LAUNCH(T, U) \
-    if (wave && p.reuseVisibility) { \
+    if (p.reuseVisibility) { \
         int rc_ = resetVisibilityQueue(ctx, stream); if (rc_) return rc_; \
         { GFX_TIMED(ctx, stream, "ris_candidates"); \
-          if (s.env.enabled) k_initialAndTemporalRIS<T, U, 1, false, true><<<grid, block, 0, stream>>>(s, f, p); \
-          else if (twoPhase) k_initialAndTemporalRIS<T, U, 1, true><<<grid, block, 0, stream>>>(s, f, p); \
-          else k_initialAndTemporalRIS<T, U, 1, false><<<grid, block, 0, stream>>>(s, f, p); } ctx->launches++; \
+          if (s.env.enabled) k_initialAndTemporalRIS<T, U, 1, true><<<grid, block, 0, stream>>>(s, f, p); \
+          else k_initialAndTemporalRIS<T, U, 1><<<grid, block, 0, stream>>>(s, f, p); } ctx->launches++; \
         rc_ = traceVisibilityQueue(ctx, stream); if (rc_) return rc_; \
         { GFX_TIMED(ctx, stream, "ris_resolve_temporal"); k_initialAndTemporalRIS<T, U, 2><<<grid, block, 0, stream>>>(s, f, p); } \
     } else { \
         { GFX_TIMED(ctx, stream, "ris_megakernel"); \
-          if (s.env.enabled) k_initialAndTemporalRIS<T, U, 0, false, true><<<grid, block, 0, stream>>>(s, f, p); \
+          if (s.env.enabled) k_initialAndTemporalRIS<T, U, 0, true><<<grid, block, 0, stream>>>(s, f, p); \
           else k_initialAndTemporalRIS<T, U, 0><<<grid, block, 0, stream>>>(s, f, p); } \
     }
     switch (pass) {
@@ -634,14 +620,14 @@ int launchReSTIR(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params
     case GFX_RESTIR_SPATIAL_UNBIASED: { GFX_TIMED(ctx, stream, "spatial_ris_unbiased"); k_spatialRIS<true><<<grid, block, 0, stream>>>(s, f, p); } break;
     case GFX_RESTIR_SHADING: {
         const bool visDone = p.reuseVisibility && (!p.enableTemporalReuse || (p.enableSpatialReuse && p.useUnbiasedEstimator));
-        if (wave && !visDone) {
+        if (!visDone) {
             int rc_ = resetVisibilityQueue(ctx, stream); if (rc_) return rc_;
             { GFX_TIMED(ctx, stream, "shading_rays"); k_shadingRays<<<grid, block, 0, stream>>>(s, f, p); } ctx->launches++;
             rc_ = traceVisibilityQueue(ctx, stream); if (rc_) return rc_;
-            { GFX_TIMED(ctx, stream, "shading"); k_shading<true><<<grid, block, 0, stream>>>(s, f, p); }
+            { GFX_TIMED(ctx, stream, "shading"); k_shading<<<grid, block, 0, stream>>>(s, f, p); }
         }
         else {
-            { GFX_TIMED(ctx, stream, "shading_megakernel"); k_shading<false><<<grid, block, 0, stream>>>(s, f, p); }
+            { GFX_TIMED(ctx, stream, "shading_megakernel"); k_shading<<<grid, block, 0, stream>>>(s, f, p); }
         }
         break;
     }

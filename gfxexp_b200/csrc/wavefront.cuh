@@ -10,11 +10,6 @@
 // is called exactly once per ray, by the lane that traced it.
 #pragma once
 #include "traverse.cuh"
-#include <cstdlib>
-
-#ifndef GFX_TRACE_FLUSH_LANES
-#define GFX_TRACE_FLUSH_LANES 16
-#endif
 
 namespace gfx {
 
@@ -47,7 +42,7 @@ GFX_D void traceWavefrontBody(const DevBvh &bvh, const float4* __restrict__ rays
     // the node step runs with most of the 32 lanes but the triangle tests inside it with few, and they issue most of the warp
     // instructions.  A lane whose traversal has ended with leaves still postponed waits
     // (`draining`) for the next flush; an occluded any-hit ray learns it at the flush.
-    constexpr int kFlushLanes = GFX_TRACE_FLUSH_LANES;
+    constexpr int kFlushLanes = 16;
     __shared__ uint32_t sharedPending[kPendingLeaves][kSmemStackThreads];
     SmemPendingLeaves pend{ &sharedPending[0][threadIdx.x], 0 };
     bool draining = false;
@@ -161,9 +156,8 @@ static inline int wavefrontGrid() {
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     // 8 x 128 threads per SM: what the any-hit kernels' 64 registers admit (H100, visibility tracer: 0.78 ms per launch at 8
-    // and at 9, 0.81 at 7; capping them at 56 registers for 9 blocks spills and costs 0.84); GFX_TRACE_BLOCKS_PER_SM overrides (A/B)
-    static const int perSm = [] { const char* e = getenv("GFX_TRACE_BLOCKS_PER_SM"); const int v = e ? atoi(e) : 0; return v > 0 && v <= 32 ? v : 8; }();
-    return sms * perSm;
+    // and at 9, 0.81 at 7; capping them at 56 registers for 9 blocks spills and costs 0.84)
+    return sms * 8;
 }
 
 } // namespace gfx

@@ -7,7 +7,7 @@ import pytest
 
 from gfxexp_b200 import abi, engine, scenes
 from tests import oracle_nrc_triwave as OW
-from tests.test_gpu_nrc import _queries, _rel_l2, _same_bits, _tile_queries, _train_targets
+from tests.test_gpu_nrc import _misaligned, _queries, _rel_l2, _same_bits, _tile_queries, _train_targets
 from tests.test_gpu_nrc_frame import SEEDED_TILE, _compare_pathtrace, _same, _seeded_preprocess
 
 pytestmark = pytest.mark.gpu
@@ -64,9 +64,10 @@ def test_encoding_is_bit_exact(gfx_ctx, oracle):
 
 
 @pytest.mark.parametrize("hidden", [2, 7])
-def test_frame_sized_batch_matches_one_tile_per_cta(gfx_ctx, oracle, monkeypatch, hidden):
-    """A batch with at least 3 tiles per CTA of the persistent kernel (double-buffered TMA stage, output staging) gives the same
-    bits as launches in which every CTA handles one tile; GFX_NRC_INFER_FUSED, a hash-grid switch, changes nothing here"""
+def test_frame_sized_batch_matches_one_tile_per_cta(gfx_ctx, oracle, hidden):
+    """A batch with at least 3 tiles per CTA gives the same bits as launches in which every CTA handles one tile: on the
+    persistent kernel (double-buffered TMA stage, output staging), and on the fused kernel, which takes a copy of the queries
+    that is not 16-byte aligned"""
     import torch
     sms = torch.cuda.get_device_properties(0).multi_processor_count
     num_tiles = max(4096, 3 * 6 * sms)
@@ -74,20 +75,18 @@ def test_frame_sized_batch_matches_one_tile_per_cta(gfx_ctx, oracle, monkeypatch
     q = _tile_queries(num_tiles, 31 + hidden)
     gnet, onet, _ = _nets(gfx_ctx, oracle, hidden, 40 + hidden)
     dq = torch.from_numpy(q).cuda()
-    whole, chunked, env = (torch.full((n, 3), float("nan"), device="cuda") for _ in range(3))
+    whole, chunked, fused = (torch.full((n, 3), float("nan"), device="cuda") for _ in range(3))
     gnet.infer(dq, whole, n)
     step = sms * 128
     for lo in range(0, n, step):
         m = min(step, n - lo)
         gnet.infer(dq[lo:lo + m], chunked[lo:lo + m], m)
-    monkeypatch.setenv("GFX_NRC_INFER_FUSED", "1")
-    gnet.infer(dq, env, n)
-    monkeypatch.delenv("GFX_NRC_INFER_FUSED")
+    gnet.infer(_misaligned(dq), fused, n)
     torch.cuda.synchronize()
-    whole, chunked, env = (t.cpu().numpy() for t in (whole, chunked, env))
+    whole, chunked, fused = (t.cpu().numpy() for t in (whole, chunked, fused))
     assert np.isfinite(whole).all()
     _same_bits(whole, chunked, "whole batch vs one tile per CTA")
-    _same_bits(env, whole, "GFX_NRC_INFER_FUSED=1")
+    _same_bits(fused, whole, "fused kernel vs persistent kernel")
     assert _rel_l2(whole, onet.infer(q)) <= 1e-3
     gnet.close()
 

@@ -1,14 +1,8 @@
 """The device's original ReSTIR DI passes on seeded synthetic frames (tests/restir_scenes.py): bit for bit against the oracle
 on every launch form - the PHASE 0 megakernel (reuseVisibility = 0), the two-phase candidate loop (<= 32 candidates), the
-lock-step loop (> 32 candidates, or an environment light) and strip launches - the GFX_MEGAKERNEL and GFX_RIS_TWO_PHASE
-switches against the default form, the saturated stream length, a 1920x1080 frame within the float64 restatement's bars
-(tests/restir_ref.py) on row windows, and the device's estimators at 512x512 against the direct-lighting integral
-(tests/restir_unbiased.py)."""
-import os
-import subprocess
-import sys
-import tempfile
-
+lock-step loop (> 32 candidates, or an environment light) and strip launches - the saturated stream length, a 1920x1080
+frame within the float64 restatement's bars (tests/restir_ref.py) on row windows, and the device's estimators at 512x512
+against the direct-lighting integral (tests/restir_unbiased.py)."""
 import numpy as np
 import pytest
 
@@ -17,7 +11,6 @@ from tests import restir_ref, restir_scenes as S
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PLANES = [(abi.BUF_RNG, 0), (abi.BUF_RESERVOIR, 0), (abi.BUF_RESERVOIR, 1), (abi.BUF_RESERVOIR_INFO, 0),
           (abi.BUF_RESERVOIR_INFO, 1), (abi.BUF_BEAUTY_ACCUM, 0)]
 # (log2 candidates, reuseVisibility, environment): two-phase, PHASE 0, lock-step by count, lock-step by the environment,
@@ -115,47 +108,6 @@ def test_stream_length_saturates_bit_exact(gfx_ctx, oracle, scenes_):
     m = dev.get(abi.BUF_RESERVOIR, 1)[1, ..., 3]
     hit = dev.get(abi.BUF_GBUFFER0, 1)[..., 0] != S.SKY
     assert not (m[hit] >> 31).any() and (m[hit] == restir_ref.M31).any()
-
-
-_CHILD = r"""
-import sys, json, numpy as np
-sys.path.insert(0, {root!r})
-from gfxexp_b200 import engine
-from tests import oracle_lib, restir_ref, restir_scenes as S
-from tests.test_gpu_restir_ref import PLANES, _cfg, _upload_scene
-out = {{}}
-ctx = engine.Context(0)
-for env, log2 in ((False, 5), (False, 6), (True, 3)):
-    sc = S.scene(env)
-    s64 = restir_ref.Scene64(sc)
-    _upload_scene(ctx, sc)
-    dev = S.DeviceSide(ctx, 33, 17)
-    S.setup_frame([dev], S.SyntheticFrames(33, 17, 6), s64, 1)
-    p = S.frame_params(sc, 33, 17, 1)
-    _cfg(p, log2, 1)
-    for pass_id in S.frame_launches(p, 1, 1, True, True):
-        dev.run(p, pass_id)
-    for buf, idx in PLANES:
-        np.save({tmp!r} + f"/{{env}}_{{log2}}_{{buf}}_{{idx}}.npy", dev.get(buf, idx))
-ctx.close()
-"""
-
-
-@pytest.mark.parametrize("switch", [("GFX_MEGAKERNEL", "1"), ("GFX_RIS_TWO_PHASE", "0")], ids=lambda s: s[0])
-def test_switches_give_the_same_bits(switch):
-    """each switch is read once per process: one child process with it set, one without, on the same frames"""
-    with tempfile.TemporaryDirectory() as tmp:
-        results = []
-        for env_extra in ({}, {switch[0]: switch[1]}):
-            d = os.path.join(tmp, str(len(results)))
-            os.makedirs(d)
-            env = {k: v for k, v in os.environ.items() if k not in ("GFX_MEGAKERNEL", "GFX_RIS_TWO_PHASE")}
-            env.update(env_extra)
-            subprocess.run([sys.executable, "-c", _CHILD.format(root=ROOT, tmp=d)], env=env, check=True, timeout=600)
-            results.append({f: np.load(os.path.join(d, f)) for f in sorted(os.listdir(d))})
-        assert results[0].keys() == results[1].keys() and len(results[0]) == 18
-        for f in results[0]:
-            assert np.array_equal(results[0][f].view(np.uint32), results[1][f].view(np.uint32)), f"{switch[0]}: {f} differs"
 
 
 def test_1080p_within_restatement_bars(gfx_ctx, scenes_):
