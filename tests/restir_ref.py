@@ -61,15 +61,18 @@ def pcg_draw(state: np.ndarray):
     return new, (out >> np.uint64(9)).astype(np.float64) * 2.0 ** -23
 
 
+def halton(base: int, i: int) -> float:
+    """the radical inverse of i in base, in float64"""
+    r, s = 0.0, 1.0
+    while i:
+        s /= base
+        r += (i % base) * s
+        i //= base
+    return r
+
+
 def neighbor_deltas() -> np.ndarray:
     """restir_di_main.cpp:1534-1540: concentricSampleDisk(Halton2(i), Halton3(i)), i < 1024"""
-    def halton(base, i):
-        r, s = 0.0, 1.0
-        while i:
-            s /= base
-            r += (i % base) * s
-            i //= base
-        return r
     u0 = np.array([halton(2, i) for i in range(1024)])
     u1 = np.array([halton(3, i) for i in range(1024)])
     return np.stack(shading_ref.concentric_sample_disk(u0, u1), -1)

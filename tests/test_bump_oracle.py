@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from gfxexp_b200 import abi, ingest, scenes
-from tests import oracle_bump
+from tests import oracle_bump, texture_ref
 
 F32 = np.float32
 
@@ -35,20 +35,6 @@ def test_atan_against_libm():
     assert abs(ys[8] - np.pi / 2) < 2e-7 and abs(ys[9] + np.pi / 2) < 2e-7
 
 
-def _bump64(n, t, b, nn):
-    """applyBumpMapping in float64 (common_device.cuh:176-203)"""
-    proj = np.hypot(n[:, 0], n[:, 1])
-    with np.errstate(divide="ignore", invalid="ignore"):
-        tilt = np.arctan(proj / n[:, 2])
-        qs, qc = np.sin(tilt / 2), np.cos(tilt / 2)
-        qx, qy, qw = -n[:, 1] / proj * qs, n[:, 0] / proj * qs, qc
-    mt = np.stack([1 - 2 * qy * qy, 2 * qx * qy, -2 * qy * qw], 1)
-    mb = np.stack([2 * qx * qy, 1 - 2 * qx * qx, 2 * qx * qw], 1)
-    M = np.stack([t, b, nn], 2)  # columns
-    out = np.concatenate([np.einsum("kij,kj->ki", M, mt), np.einsum("kij,kj->ki", M, mb), np.einsum("kij,kj->ki", M, n)], 1)
-    return np.where((proj < 1e-3)[:, None], np.concatenate([t, b, nn], 1), out)
-
-
 def _random_frames(rng, k):
     q, _ = np.linalg.qr(rng.normal(size=(k, 3, 3)))
     return q[:, :, 0], q[:, :, 1], q[:, :, 2]
@@ -67,7 +53,7 @@ def test_apply_bump_mapping_against_float64(bumped):
     inp = np.concatenate([n, t, b, nn], 1).astype(F32)
     got = _query(oscene, 1, 0, inp, 9).astype(np.float64)
     i64 = inp.astype(np.float64)
-    want = _bump64(i64[:, 0:3], i64[:, 3:6], i64[:, 6:9], i64[:, 9:12])
+    want = texture_ref.apply_bump_mapping(i64[:, 0:3], i64[:, 3:6], i64[:, 6:9], i64[:, 9:12])
     assert np.abs(got - want).max() < 2e-5
     small = slice(k // 4, k // 4 + 100)
     assert np.array_equal(got[small], inp[small, 3:12].astype(np.float64))  # bit for bit: returned as it came
@@ -94,7 +80,7 @@ def test_default_texel_tilts_every_material(bumped):
     uv = np.random.default_rng(1).uniform(-3, 3, (64, 2)).astype(F32)
     n = _query(oscene, 0, m, uv, 3)
     texel = np.array([[[F32(127) / F32(255), F32(127) / F32(255), 1, 1]]], dtype=F32)
-    blend, _ = _fetch_repeat32(texel, uv[:, 0], uv[:, 1])  # the software filter's four taps of the one texel
+    blend, _ = texture_ref.fetch_repeat(texel, uv[:, 0], uv[:, 1])  # the software filter's four taps of the one texel
     want = F32(2) * blend[:, :3] - F32(1)
     want[:, 1] = -want[:, 1]
     assert np.array_equal(n, want)
@@ -102,32 +88,6 @@ def test_default_texel_tilts_every_material(bumped):
     frame = _query(oscene, 1, 0, np.concatenate([n[:1], [[1, 0, 0, 0, 1, 0, 0, 0, 1]]], 1), 9)
     tilt = np.arccos(frame[0, 8] / np.linalg.norm(frame[0, 6:9]))
     assert abs(tilt - np.arctan(np.sqrt(2) / 255)) < 1e-5 and abs(np.sqrt(2) / 255 - 0.0055) < 1e-4
-
-
-def _fetch_repeat32(tex, u, v):
-    """textureFetchRepeat in float32 (fixed 8-bit fraction, the four texels blended in order)"""
-    H, W = tex.shape[:2]
-    xB = (u - np.floor(u)) * F32(W) - F32(0.5)
-    yB = (v - np.floor(v)) * F32(H) - F32(0.5)
-    fx, fy = np.floor(xB), np.floor(yB)
-    a = np.floor((xB - fx) * F32(256) + F32(0.5)) * F32(1 / 256)
-    b = np.floor((yB - fy) * F32(256) + F32(0.5)) * F32(1 / 256)
-    ix, iy = fx.astype(np.int64), fy.astype(np.int64)
-    x0, x1, y0, y1 = ix % W, (ix + 1) % W, iy % H, (iy + 1) % H
-    w00, w10, w01, w11 = (F32(1) - a) * (F32(1) - b), a * (F32(1) - b), (F32(1) - a) * b, a * b
-    return (w00[:, None] * tex[y0, x0] + w10[:, None] * tex[y0, x1] + w01[:, None] * tex[y1, x0] + w11[:, None] * tex[y1, x1]).astype(F32), (x0, x1, y0, y1)
-
-
-def _gather_indices(tex, u, v):
-    """the footprint of tex2Dgather: floor(xB), one texel on when the fraction is above 255.5 / 256, wrapped"""
-    H, W = tex.shape[:2]
-    out = []
-    for c, n in ((u, W), (v, H)):
-        xB = (c - np.floor(c)) * F32(n) - F32(0.5)
-        fx = np.floor(xB)
-        i = fx.astype(np.int64) + ((xB - fx) * F32(256) > F32(255.5))
-        out += [i % n, (i + 1) % n]
-    return out[0], out[1], out[2], out[3]
 
 
 def test_normal_decode_and_height_gather_against_numpy(bumped):
@@ -145,8 +105,8 @@ def test_normal_decode_and_height_gather_against_numpy(bumped):
         tex = scene.textures[tex_index]
         got_n = _query(oscene, 0, m, uv, 3)
         got_g = _query(oscene, 2, m, uv, 4)
-        blend, _ = _fetch_repeat32(tex, u, v)
-        x0, x1, y0, y1 = _gather_indices(tex, u, v)
+        blend, _ = texture_ref.fetch_repeat(tex, u, v)
+        x0, x1, y0, y1 = texture_ref.gather_indices(tex, u, v)
         want_g = np.stack([tex[y1, x0, 0], tex[y1, x1, 0], tex[y0, x1, 0], tex[y0, x0, 0]], 1)
         assert np.array_equal(got_g, want_g)
         if kind == abi.BUMP_NORMAL_MAP:
