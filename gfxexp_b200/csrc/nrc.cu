@@ -15,8 +15,9 @@
 // memory, pre-arranged in the core-matrix layout by k_nrcPrepWeights.  No activation ever touches HBM:
 // the compulsory traffic is 56 B in + 12 B out per query (SURVEY.md §8d).
 //
-// Training (4 x 16 384 samples per frame) is latency-bound and runs on CUDA cores: one block = 128
-// samples, weights and activations in shared memory, dW reduced per block then atomically added.
+// Training (4 x 16 384 samples per frame) is latency-bound: one block = 128 samples, weights and activations in shared
+// memory, every matrix product on wgmma (k_nrcTrainTc) for 1..3 hidden layers; deeper networks, whose activation tiles do
+// not fit, train on CUDA cores (k_nrcTrain).  Weight gradients are accumulated with 64-bit fixed-point atomics.
 //
 // Both of NeuralRadianceCache::initialize's position encodings are built (gfx_nrc_create_with_encoding): the hash grid above,
 // and the triangle wave (triangle_wave.h:47-81), which has no parameters and no grid stage - k_nrcInferMlp<kEncTriangleWave> is
@@ -90,55 +91,63 @@ GFX_D uint32_t nrcWrap(uint32_t index, uint32_t size) {
     return index < size ? index : index % size;
 }
 
-// grid_index (grid.h:76-111) for the 8 corners of one cell: the per-axis terms of the dense stride sum or of the
-// coherent prime hash are computed once, a corner is one 3-input add/xor plus the wrap. Everything that depends only
-// on the level is warp-uniform.
-struct NrcCellIndexer {
+// grid_index's per-axis multipliers of one level (grid.h:76-111): the dense strides (0 for an axis the table does not reach),
+// or the coherent hash's primes when the dense grid outgrows the table.  Returns whether the level is hashed.
+GFX_D bool nrcLevelMultipliers(const NrcLevel &lv, uint32_t (&mul)[3]) {
+    uint32_t stride = 1;
+    uint32_t strides[3];
+    bool used[3];
+#pragma unroll
+    for (uint32_t dim = 0; dim < 3; ++dim) {
+        used[dim] = stride <= lv.hashmapSize;
+        strides[dim] = stride;
+        if (used[dim])
+            stride *= lv.resolution;
+    }
+    const bool hashed = lv.hashmapSize < stride;
+    const uint32_t primes[3] = { 1u, 2654435761u, 805459861u };
+#pragma unroll
+    for (uint32_t dim = 0; dim < 3; ++dim)
+        mul[dim] = hashed ? primes[dim] : (used[dim] ? strides[dim] : 0u);
+    return hashed;
+}
+
+// The cell of one level that a position falls in: pos_fract (common_device.h:425-431), then grid_index for its 8 corners.
+// The per-axis terms of the dense stride sum or of the coherent prime hash are computed once, a corner is one 3-input add/xor
+// plus the wrap.  Everything that depends only on the level is warp-uniform.  Corner bit d of idx selects the upper neighbour
+// along axis d.
+struct NrcCell {
+    float frac[3];
     uint32_t term[3][2];
     uint32_t size;
     bool hashed;
-    GFX_D NrcCellIndexer(const NrcLevel &lv, const uint32_t posGrid[3]) {
+    GFX_D NrcCell(const NrcLevel &lv, const float p[3]) {
+        uint32_t mul[3];
+        hashed = nrcLevelMultipliers(lv, mul);
         size = lv.hashmapSize;
-        uint32_t stride = 1;
-        uint32_t strides[3];
-        bool used[3];
 #pragma unroll
-        for (uint32_t dim = 0; dim < 3; ++dim) {
-            used[dim] = stride <= lv.hashmapSize;
-            strides[dim] = stride;
-            if (used[dim])
-                stride *= lv.resolution;
-        }
-        hashed = lv.hashmapSize < stride;
-        const uint32_t primes[3] = { 1u, 2654435761u, 805459861u };
-#pragma unroll
-        for (uint32_t dim = 0; dim < 3; ++dim) {
-            const uint32_t m = hashed ? primes[dim] : (used[dim] ? strides[dim] : 0u);
-            term[dim][0] = posGrid[dim] * m;
-            term[dim][1] = term[dim][0] + m;
+        for (uint32_t d = 0; d < 3; ++d) {
+            frac[d] = p[d] * lv.scale + 0.5f;
+            const int tmp = (int)floorf(frac[d]);
+            frac[d] -= (float)tmp;
+            term[d][0] = (uint32_t)tmp * mul[d];
+            term[d][1] = term[d][0] + mul[d];
         }
     }
-    // corner bit d of idx selects posGrid[d] + 1; returns the index of the first of the two features
-    GFX_D uint32_t corner(uint32_t idx) const {
+    // the corner's entry of the level's table (two features)
+    GFX_D uint32_t entry(uint32_t idx) const {
         const uint32_t a = term[0][idx & 1u], b = term[1][(idx >> 1) & 1u], c = term[2][(idx >> 2) & 1u];
-        return nrcWrap(hashed ? (a ^ b ^ c) : (a + b + c), size) * 2u;
+        return nrcWrap(hashed ? (a ^ b ^ c) : (a + b + c), size);
+    }
+    // the corner's trilinear weight
+    GFX_D float weight(uint32_t idx) const {
+        float w = 1;
+#pragma unroll
+        for (uint32_t d = 0; d < 3; ++d)
+            w *= (idx & (1u << d)) == 0 ? 1 - frac[d] : frac[d];
+        return w;
     }
 };
-
-GFX_D uint32_t nrcGridIndex(const NrcLevel &lv, const uint32_t pos[3]) { // grid.h:76-111
-    uint32_t stride = 1;
-    uint32_t index = 0;
-#pragma unroll
-    for (uint32_t dim = 0; dim < 3; ++dim) {
-        if (stride <= lv.hashmapSize) {
-            index += pos[dim] * stride;
-            stride *= lv.resolution;
-        }
-    }
-    if (lv.hashmapSize < stride)
-        index = (pos[0] * 1u) ^ (pos[1] * 2654435761u) ^ (pos[2] * 805459861u);
-    return (index % lv.hashmapSize) * 2u;
-}
 
 // OneBlob: 5 dims x 4 bins -> features 32..51, identity 52..57, ones 58..63 (q = the 14 query floats; q[0..2] unused)
 GFX_D void nrcEncodeTail(const float* q, __half* tail) {
@@ -174,40 +183,24 @@ GFX_D void nrcEncode(const NrcLevels &levels, const __half* __restrict__ table, 
     for (uint32_t d = 0; d < kInputDims; ++d)
         q[d] = in[d];
     __half feat[8];
-    // One level at a time, the 8 gathers interleaved with their index arithmetic: the encoder is bound by the L1's
-    // divergent-gather rate, not by issue.
+    // One level at a time: the encoder is bound by the L1's divergent-gather rate, not by issue.  The 8 gathers are all
+    // issued before the blend uses them: a corner's wrap may branch, and a load cannot move above a branch, so a blend step
+    // between them would wait for each gather in turn.
 #pragma unroll 1
     for (uint32_t l = 0; l < kLevels; ++l) {
         const NrcLevel lv = levels.l[l];
         const __half2* grid = reinterpret_cast<const __half2*>(table + (size_t)lv.offset * 2);
-        float pos[3];
-        uint32_t posGrid[3];
+        const NrcCell cell(lv, q);
+        __half2 v[8];
 #pragma unroll
-        for (uint32_t d = 0; d < 3; ++d) {
-            pos[d] = q[d] * lv.scale + 0.5f;
-            const int tmp = (int)floorf(pos[d]);
-            posGrid[d] = (uint32_t)tmp;
-            pos[d] -= (float)tmp;
-        }
+        for (uint32_t idx = 0; idx < 8; ++idx)
+            v[idx] = __ldg(grid + cell.entry(idx));
         __half r0 = __float2half(0.0f), r1 = __float2half(0.0f);
 #pragma unroll
         for (uint32_t idx = 0; idx < 8; ++idx) {
-            float weight = 1;
-            uint32_t local[3];
-#pragma unroll
-            for (uint32_t d = 0; d < 3; ++d) {
-                if ((idx & (1u << d)) == 0) {
-                    weight *= 1 - pos[d];
-                    local[d] = posGrid[d];
-                }
-                else {
-                    weight *= pos[d];
-                    local[d] = posGrid[d] + 1;
-                }
-            }
-            const __half2 v = __ldg(grid + (nrcGridIndex(lv, local) >> 1));
-            r0 = __float2half(__half2float(r0) + __half2float(__float2half(weight * __low2float(v))));
-            r1 = __float2half(__half2float(r1) + __half2float(__float2half(weight * __high2float(v))));
+            const float weight = cell.weight(idx);
+            r0 = __float2half(__half2float(r0) + __half2float(__float2half(weight * __low2float(v[idx]))));
+            r1 = __float2half(__half2float(r1) + __half2float(__float2half(weight * __high2float(v[idx]))));
         }
         feat[(l & 3) * 2 + 0] = r0;
         feat[(l & 3) * 2 + 1] = r1;
@@ -431,12 +424,21 @@ GFX_D void mbarWait(uint64_t* bar, uint32_t phase) {
         :: "r"(smemU32(bar)), "r"(phase) : "memory");
 }
 GFX_D void fenceProxyAsync() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+GFX_D void bulkLoad(void* smemDst, const void* globalSrc, uint32_t bytes, uint64_t* bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                 :: "r"(smemU32(smemDst)), "l"(globalSrc), "r"(bytes), "r"(smemU32(bar)) : "memory");
+}
+GFX_D void mbarExpectTx(uint64_t* bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smemU32(bar)), "r"(bytes) : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------
-// k_nrcPrepWeights: EMA MLP weights [out][in] -> per-layer K-major core-matrix blobs:
+// k_nrcPrepWeights: MLP weights W_l [out][in] -> per-layer K-major core-matrix blobs of W_l ([N x 64]):
 //   byte offset(layer, n, k) = layerBase + (k / 8) * (N * 16) + n * 16 + (k % 8) * 2
+// and, for training (blobT not null), of W_l^T ([64 x K], 64 rows per K-chunk)
 // ---------------------------------------------------------------------------------------------
-__global__ void k_nrcPrepWeights(const __half* __restrict__ w, uint32_t numHiddenLayers, __half* __restrict__ blob) {
+__global__ void k_nrcPrepWeights(const __half* __restrict__ w, uint32_t numHiddenLayers, __half* __restrict__ blob,
+                                 __half* __restrict__ blobT) {
     const uint32_t total = numHiddenLayers * kWidth * kWidth + kPaddedOutput * kWidth;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
         uint32_t layer = i / (kWidth * kWidth), rem = i % (kWidth * kWidth), N = kWidth;
@@ -446,8 +448,9 @@ __global__ void k_nrcPrepWeights(const __half* __restrict__ w, uint32_t numHidde
             N = kPaddedOutput;
         }
         const uint32_t n = rem / kWidth, k = rem % kWidth;
-        const uint32_t dst = layer * kWidth * kWidth + (k / 8) * (N * 8) + n * 8 + (k % 8);
-        blob[dst] = w[i];
+        blob[layer * kWidth * kWidth + (k / 8) * (N * 8) + n * 8 + (k % 8)] = w[i];
+        if (blobT)
+            blobT[layer * kWidth * kWidth + (n / 8) * (kWidth * 8) + k * 8 + (n % 8)] = w[i];
     }
 }
 
@@ -456,6 +459,62 @@ __global__ void k_nrcPrepWeights(const __half* __restrict__ w, uint32_t numHidde
 // ---------------------------------------------------------------------------------------------
 constexpr uint32_t kTileRows = 128;
 constexpr uint32_t kATileBytes = kTileRows * kWidth * 2; // 16 KB: 8 K-chunks x 128 rows x 16 B
+
+// query q encoded into row `row` of a [128 x 64] K-major tile (chunk c of 8 features at c * 2048 + row * 16), zeros past numData
+template <uint32_t kEnc>
+GFX_D void encodeTileRow(const NrcLevels &levels, const __half* __restrict__ table, const float* __restrict__ input, uint32_t q,
+                         uint32_t numData, uint8_t* tile, uint32_t row) {
+    if (q < numData) {
+        nrcEncodeQuery<kEnc>(levels, table, input + (size_t)q * kInputDims, [&](uint32_t c, const __half* f) {
+            *reinterpret_cast<uint4*>(tile + c * (kTileRows * 16) + row * 16) = packHalf8(f);
+        });
+    }
+    else {
+#pragma unroll
+        for (uint32_t c = 0; c < 8; ++c)
+            *reinterpret_cast<uint4*>(tile + c * (kTileRows * 16) + row * 16) = make_uint4(0, 0, 0, 0);
+    }
+}
+
+// The MLP over one 128-row tile whose inputs are in sA (overwritten by the hidden activations): per hidden layer mlpLayer64
+// and the ReLU epilogue, then the 16-wide output layer, whose accumulators go to out(acc)
+template <typename Out>
+GFX_D void mlpTile(uint8_t* sA, uint32_t wAddr, uint32_t numHiddenLayers, uint32_t tid, Out out) {
+    const uint32_t aAddr = smemU32(sA);
+    for (uint32_t layer = 0; layer <= numHiddenLayers; ++layer) {
+        // make the generic-proxy writes of sA (and of the weights) visible to the tensor core
+        fenceProxyAsync();
+        __syncthreads();
+        const uint32_t wLayer = wAddr + layer * kWidth * kWidth * 2;
+        if (layer < numHiddenLayers) {
+            float acc[2][32];
+            mlpLayer64(acc, aAddr, kTileRows * 16, wLayer, kWidth / 16);
+            __syncthreads(); // every warp's MMAs have read the A tile before it is overwritten
+            storeReluTile(acc, sA, tid);
+        }
+        else {
+            float acc[2][8];
+            mlpLayer16(acc, aAddr, kTileRows * 16, wLayer);
+            out(acc);
+        }
+    }
+}
+
+// the network outputs (columns 0..2) of the output layer's accumulators: write(tile row, column, value); they are held by
+// lanes with l % 4 < 2
+template <typename Write>
+GFX_D void forEachOutput(const float (&acc)[2][8], uint32_t tid, Write write) {
+#pragma unroll
+    for (uint32_t h = 0; h < 2; ++h)
+#pragma unroll
+        for (uint32_t i = 0; i < 2; ++i)
+#pragma unroll
+            for (uint32_t e = 0; e < 2; ++e) {
+                const uint32_t r = h * 64 + fragRow(tid, i), c = fragCol(tid, 0) + e;
+                if (c < kOutputDims)
+                    write(r, c, acc[h][2 * i + e]);
+            }
+}
 
 template <uint32_t kEnc>
 __global__ void __launch_bounds__(128) k_nrcInfer(NrcLevels levels, const __half* __restrict__ table,
@@ -476,51 +535,19 @@ __global__ void __launch_bounds__(128) k_nrcInfer(NrcLevels levels, const __half
     for (uint32_t i = tid; i < weightBytes / 16; i += 128)
         reinterpret_cast<uint4*>(sW)[i] = __ldg(ummaWeights + i);
 
-    const uint32_t aAddr = smemU32(sA);
     const uint32_t wAddr = smemU32(sW);
 
     const uint32_t numTiles = (numData + kTileRows - 1) / kTileRows;
     for (uint32_t tile = blockIdx.x; tile < numTiles; tile += gridDim.x) {
-        const uint32_t row = tile * kTileRows + tid;
-        // ---- encode this thread's query into the A tile: chunk c at c * 2048 + row * 16
-        if (row < numData) {
-            nrcEncodeQuery<kEnc>(levels, table, input + (size_t)row * kInputDims, [&](uint32_t c, const __half* f) {
-                *reinterpret_cast<uint4*>(sA + c * (kTileRows * 16) + tid * 16) = packHalf8(f);
+        encodeTileRow<kEnc>(levels, table, input, tile * kTileRows + tid, numData, sA, tid);
+        mlpTile(sA, wAddr, numHiddenLayers, tid, [&](const float (&acc)[2][8]) {
+            // trim_and_cast_from: half output -> float
+            forEachOutput(acc, tid, [&](uint32_t r, uint32_t c, float v) {
+                const uint32_t row = tile * kTileRows + r;
+                if (row < numData)
+                    output[(size_t)row * kOutputDims + c] = __half2float(__float2half(v));
             });
-        }
-        else {
-#pragma unroll
-            for (uint32_t c = 0; c < 8; ++c)
-                *reinterpret_cast<uint4*>(sA + c * (kTileRows * 16) + tid * 16) = make_uint4(0, 0, 0, 0);
-        }
-
-        for (uint32_t layer = 0; layer <= numHiddenLayers; ++layer) {
-            // make the generic-proxy writes of sA (and of the weights) visible to the tensor core
-            fenceProxyAsync();
-            __syncthreads();
-            const uint32_t wLayer = wAddr + layer * kWidth * kWidth * 2;
-            if (layer < numHiddenLayers) {
-                float acc[2][32];
-                mlpLayer64(acc, aAddr, kTileRows * 16, wLayer, kWidth / 16);
-                __syncthreads(); // every warp's MMAs have read the A tile before it is overwritten
-                storeReluTile(acc, sA, tid);
-            }
-            else {
-                float acc[2][8];
-                mlpLayer16(acc, aAddr, kTileRows * 16, wLayer);
-                // trim_and_cast_from: half output -> float; columns 0..2 are held by lanes with l % 4 < 2
-#pragma unroll
-                for (uint32_t h = 0; h < 2; ++h)
-#pragma unroll
-                    for (uint32_t i = 0; i < 2; ++i)
-#pragma unroll
-                        for (uint32_t e = 0; e < 2; ++e) {
-                            const uint32_t r = tile * kTileRows + h * 64 + fragRow(tid, i), c = fragCol(tid, 0) + e;
-                            if (c < kOutputDims && r < numData)
-                                output[(size_t)r * kOutputDims + c] = __half2float(__float2half(acc[h][2 * i + e]));
-                        }
-            }
-        }
+        });
         // all warps are done with the A tile before the next tile overwrites it
         __syncthreads();
     }
@@ -551,14 +578,6 @@ __global__ void k_nrcPackPositions(const float* __restrict__ input, float4* __re
     }
 }
 
-GFX_D void bulkLoad(void* smemDst, const void* globalSrc, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 :: "r"(smemU32(smemDst)), "l"(globalSrc), "r"(bytes), "r"(smemU32(bar)) : "memory");
-}
-GFX_D void mbarExpectTx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smemU32(bar)), "r"(bytes) : "memory");
-}
-
 constexpr uint32_t kEncodeThreads = 1024;
 constexpr uint32_t kTileFeatureBytes = kLevels * 128 * 4; // 8 KB per 128-query tile: [level][row] half2
 
@@ -584,24 +603,13 @@ __global__ void __launch_bounds__(kEncodeThreads, 1) k_nrcGridEncode(NrcLevels l
     mbarWait(&bar, 0);
     __half2* grid = reinterpret_cast<__half2*>(smem);
 
-    // level constants of grid_index (grid.h:76-111), hoisted: dense levels add strides, hashed levels xor prime products
-    uint32_t stride = 1, strides[3];
-    bool used[3];
-#pragma unroll
-    for (uint32_t dim = 0; dim < 3; ++dim) {
-        used[dim] = stride <= lv.hashmapSize;
-        strides[dim] = stride;
-        if (used[dim])
-            stride *= lv.resolution;
-    }
-    const bool hashed = lv.hashmapSize < stride;
-
     // Dense levels index x + y * res + z * res^2 with res a multiple of 16: the queries of a warp are consecutive pixels, whose
     // positions typically run along ONE grid axis, so along y or z all 32 lanes would hit the same shared-memory bank (the dense
     // levels' CTAs would take twice as long as the hashed ones' and set the kernel's duration).  Entries are therefore
     // permuted inside each aligned row of 32: entry i lives at i ^ swz(i >> 5), swz(r) = (r ^ (r >> 5)) & 31 - y and z
     // neighbours land in different banks.  Hashed levels are spread by the hash already.
-    const bool swizzle = !hashed && (lv.hashmapSize & 31u) == 0u;
+    uint32_t mul[3];
+    const bool swizzle = !nrcLevelMultipliers(lv, mul) && (lv.hashmapSize & 31u) == 0u;
     const uint32_t swzMask = swizzle ? 31u : 0u;
     if (swizzle) {
         const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5, numRows = lv.hashmapSize >> 5;
@@ -619,37 +627,15 @@ __global__ void __launch_bounds__(kEncodeThreads, 1) k_nrcGridEncode(NrcLevels l
     const uint32_t qBegin = min(replica * tilesPer, numTiles) * 128u;
     const uint32_t qEnd = min(min((replica + 1) * tilesPer, numTiles) * 128u, numData);
 
-    const uint32_t primes[3] = { 1u, 2654435761u, 805459861u };
-    uint32_t mul[3];
-#pragma unroll
-    for (uint32_t dim = 0; dim < 3; ++dim)
-        mul[dim] = hashed ? primes[dim] : (used[dim] ? strides[dim] : 0u);
-    const uint32_t size = lv.hashmapSize;
-    const bool pow2 = (size & (size - 1u)) == 0u;
-
     for (uint32_t q = qBegin + threadIdx.x; q < qEnd; q += kEncodeThreads) {
         const float4 p = __ldg(positions + q);
         const float in[3] = { p.x, p.y, p.z };
-        float pos[3];
-        uint32_t term[3][2];
-#pragma unroll
-        for (uint32_t d = 0; d < 3; ++d) { // pos_fract, common_device.h:425-431
-            pos[d] = in[d] * lv.scale + 0.5f;
-            const int tmp = (int)floorf(pos[d]);
-            pos[d] -= (float)tmp;
-            term[d][0] = (uint32_t)tmp * mul[d];
-            term[d][1] = term[d][0] + mul[d];
-        }
+        const NrcCell cell(lv, in);
         __half2 r = __floats2half2_rn(0.0f, 0.0f);
 #pragma unroll
         for (uint32_t idx = 0; idx < 8; ++idx) {
-            float weight = 1;
-#pragma unroll
-            for (uint32_t d = 0; d < 3; ++d)
-                weight *= (idx & (1u << d)) == 0 ? 1 - pos[d] : pos[d];
-            const uint32_t a = term[0][idx & 1u], b = term[1][(idx >> 1) & 1u], c = term[2][(idx >> 2) & 1u];
-            uint32_t index = hashed ? (a ^ b ^ c) : (a + b + c);
-            index = pow2 ? (index & (size - 1u)) : (index < size ? index : index % size);
+            const float weight = cell.weight(idx);
+            uint32_t index = cell.entry(idx);
             index ^= ((index >> 5) ^ (index >> 10)) & swzMask;
             const float2 v = __half22float2(grid[index]);
             // result += (half)(weight * (float)value) in half precision (grid.h:233-238); __hadd2 rounds the exact sum once,
@@ -691,7 +677,7 @@ __global__ void __launch_bounds__(128) k_nrcInferMlp(const uint4* __restrict__ u
     const uint32_t numTiles = numData / kTileRows;
 
     auto requestTile = [&](uint32_t tile, uint32_t b) { // thread 0 only
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+        fenceProxyAsync();
         mbarExpectTx(&stageBar[b], (uint32_t)sizeof(Stage));
         bulkLoad(stage[b].query, input + (size_t)tile * 128 * kInputDims, 128 * kInputDims * 4, &stageBar[b]);
         if constexpr (kEnc == kEncHashGrid)
@@ -709,7 +695,6 @@ __global__ void __launch_bounds__(128) k_nrcInferMlp(const uint4* __restrict__ u
         reinterpret_cast<uint4*>(sW)[i] = __ldg(ummaWeights + i);
     __syncthreads();
 
-    const uint32_t aAddr = smemU32(sA);
     const uint32_t wAddr = smemU32(sW);
     uint32_t stagePhase0 = 0, stagePhase1 = 0, buf = 0;
 
@@ -759,37 +744,14 @@ __global__ void __launch_bounds__(128) k_nrcInferMlp(const uint4* __restrict__ u
                 *reinterpret_cast<uint4*>(sA + (4 + c) * (kTileRows * 16) + tid * 16) = packHalf8(tail + 8 * c);
         }
 
-        for (uint32_t layer = 0; layer <= numHiddenLayers; ++layer) {
-            // make the generic-proxy writes of sA (and of the weights) visible to the tensor core
-            fenceProxyAsync();
+        mlpTile(sA, wAddr, numHiddenLayers, tid, [&](const float (&acc)[2][8]) {
+            // the previous tile's bulk store must have read sOut before it is overwritten
+            if (tid == 0)
+                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
             __syncthreads();
-            const uint32_t wLayer = wAddr + layer * kWidth * kWidth * 2;
-            if (layer < numHiddenLayers) {
-                float acc[2][32];
-                mlpLayer64(acc, aAddr, kTileRows * 16, wLayer, kWidth / 16);
-                __syncthreads(); // every warp's MMAs have read the A tile before it is overwritten
-                storeReluTile(acc, sA, tid);
-            }
-            else {
-                float acc[2][8];
-                mlpLayer16(acc, aAddr, kTileRows * 16, wLayer);
-                // the previous tile's bulk store must have read sOut before it is overwritten
-                if (tid == 0)
-                    asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                __syncthreads();
-                // trim_and_cast_from: half output -> float; columns 0..2 are held by lanes with l % 4 < 2
-#pragma unroll
-                for (uint32_t h = 0; h < 2; ++h)
-#pragma unroll
-                    for (uint32_t i = 0; i < 2; ++i)
-#pragma unroll
-                        for (uint32_t e = 0; e < 2; ++e) {
-                            const uint32_t r = h * 64 + fragRow(tid, i), c = fragCol(tid, 0) + e;
-                            if (c < kOutputDims)
-                                sOut[r * kOutputDims + c] = __half2float(__float2half(acc[h][2 * i + e]));
-                        }
-            }
-        }
+            // trim_and_cast_from: half output -> float
+            forEachOutput(acc, tid, [&](uint32_t r, uint32_t c, float v) { sOut[r * kOutputDims + c] = __half2float(__float2half(v)); });
+        });
         // all warps are done reading the A tile / the stage and writing sOut before the next tile overwrites them
         fenceProxyAsync();
         __syncthreads();
@@ -803,39 +765,35 @@ __global__ void __launch_bounds__(128) k_nrcInferMlp(const uint4* __restrict__ u
         asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
 }
 
-// test hook: the 64 encoded halves per query as the split pipeline produces them (pack -> grid encode -> tail)
+// test hook: the 64 encoded halves per query as k_nrcInferMlp assembles them - hash grid: the features of pack -> grid encode,
+// then the tail; triangle wave: nrcEncodeTriWave
+template <uint32_t kEnc>
 __global__ void k_nrcAssembleEncoding(const float* __restrict__ input, const __half2* __restrict__ features, uint32_t numData,
                                       __half* __restrict__ out) {
     const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= numData)
         return;
     __half* o = out + (size_t)q * 64;
-    for (uint32_t l = 0; l < kLevels; ++l) {
-        const __half2 v = features[((size_t)(q >> 7) * kLevels + l) * 128u + (q & 127u)];
-        o[2 * l] = __low2half(v);
-        o[2 * l + 1] = __high2half(v);
+    float qv[kInputDims];
+    for (uint32_t d = 0; d < kInputDims; ++d)
+        qv[d] = input[(size_t)q * kInputDims + d];
+    if constexpr (kEnc == kEncHashGrid) {
+        for (uint32_t l = 0; l < kLevels; ++l) {
+            const __half2 v = features[((size_t)(q >> 7) * kLevels + l) * 128u + (q & 127u)];
+            o[2 * l] = __low2half(v);
+            o[2 * l + 1] = __high2half(v);
+        }
+        __half tail[32];
+        nrcEncodeTail(qv, tail);
+        for (uint32_t k = 0; k < 32; ++k)
+            o[32 + k] = tail[k];
     }
-    float qv[kInputDims];
-    for (uint32_t d = 0; d < kInputDims; ++d)
-        qv[d] = input[(size_t)q * kInputDims + d];
-    __half tail[32];
-    nrcEncodeTail(qv, tail);
-    for (uint32_t k = 0; k < 32; ++k)
-        o[32 + k] = tail[k];
-}
-
-// test hook: the triangle-wave network's 64 inputs per query, by the nrcEncodeTriWave the inference kernels run
-__global__ void k_nrcTriWaveEncoding(const float* __restrict__ input, uint32_t numData, __half* __restrict__ out) {
-    const uint32_t q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= numData)
-        return;
-    float qv[kInputDims];
-    for (uint32_t d = 0; d < kInputDims; ++d)
-        qv[d] = input[(size_t)q * kInputDims + d];
-    nrcEncodeTriWave(qv, [&](uint32_t c, const __half* f) {
-        for (uint32_t e = 0; e < 8; ++e)
-            out[(size_t)q * 64 + c * 8 + e] = f[e];
-    });
+    else {
+        nrcEncodeTriWave(qv, [&](uint32_t c, const __half* f) {
+            for (uint32_t e = 0; e < 8; ++e)
+                o[c * 8 + e] = f[e];
+        });
+    }
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -848,6 +806,61 @@ GFX_D void atomicAddFixed(unsigned long long* p, float v) {
 }
 GFX_D float fixedToFloat(unsigned long long v) {
     return (float)((double)(long long)v * (1.0 / 1073741824.0));
+}
+
+// RelativeL2Luminance (relative_l2_luminance.h:41-88) of one sample with network output o[0..2]: returns its loss term and
+// writes dL/dy, loss-scaled and fp16 like tiny-cuda-nn's backward buffers, to d[0..15] (zero for the padding and for invalid
+// samples)
+GFX_D float nrcRelativeL2Luminance(const __half* o, const float* __restrict__ target, bool valid, uint32_t numData, __half* d) {
+    float loss = 0.0f;
+    const uint32_t nTotal = numData * kOutputDims;
+    const float r = __half2float(o[0]), g = __half2float(o[1]), b = __half2float(o[2]);
+    const float luminance = 0.299f * r + 0.587f * g + 0.114f * b;
+    const float denom = luminance * luminance + 0.01f;
+#pragma unroll
+    for (uint32_t k = 0; k < kPaddedOutput; ++k) {
+        float gr = 0.0f;
+        if (k < kOutputDims && valid) {
+            const float difference = __half2float(o[k]) - target[k];
+            loss += difference * difference / denom / nTotal;
+            gr = kLossScale * (2 * difference / denom) / nTotal;
+        }
+        d[k] = __float2half(gr);
+    }
+    return loss;
+}
+
+// hash-grid backward (kernel_grid_backward, grid.h:306-429) of one sample at position in[0..2]: the gradients of the first 32
+// network inputs, grad(2 l + e) for feature e of level l, scattered to the corners of each level's cell
+template <typename Grad>
+GFX_D void nrcGridBackward(const NrcLevels &levels, const float* __restrict__ in, Grad grad, unsigned long long* gGrid) {
+    const float p[3] = { in[0], in[1], in[2] };
+    for (uint32_t l = 0; l < kLevels; ++l) {
+        const NrcLevel lv = levels.l[l];
+        const float g0 = grad(l * 2 + 0), g1 = grad(l * 2 + 1);
+        if (g0 == 0.0f && g1 == 0.0f)
+            continue;
+        const NrcCell cell(lv, p);
+#pragma unroll
+        for (uint32_t idx = 0; idx < 8; ++idx) {
+            const float weight = cell.weight(idx);
+            const uint32_t gi = lv.offset * 2 + cell.entry(idx) * 2;
+            atomicAddFixed(gGrid + gi, weight * g0);
+            atomicAddFixed(gGrid + gi + 1, weight * g1);
+        }
+    }
+}
+
+// the 128-thread block's loss terms, summed per warp and then over the 4 warps, added to *lossOut
+GFX_D void nrcBlockLoss(float localLoss, float* lossOut) {
+    __shared__ float sLoss[4];
+    for (int off = 16; off > 0; off >>= 1)
+        localLoss += __shfl_xor_sync(0xFFFFFFFFu, localLoss, off);
+    if ((threadIdx.x & 31) == 0)
+        sLoss[threadIdx.x >> 5] = localLoss;
+    __syncthreads();
+    if (threadIdx.x == 0)
+        atomicAdd(lossOut, sLoss[0] + sLoss[1] + sLoss[2] + sLoss[3]);
 }
 
 constexpr uint32_t kRowStride = 66; // halves per activation row in shared memory (conflict-free rows)
@@ -864,7 +877,6 @@ __global__ void __launch_bounds__(128) k_nrcTrain(NrcLevels levels, const __half
     __half* sW = reinterpret_cast<__half*>(smem);                              // numMatrixWeights
     __half* sAct = sW + numMatrixWeights;                                      // (H + 1) x 128 x kRowStride
     __half* sD = sAct + (size_t)(H + 1) * 128 * kRowStride;                    // 128 x kRowStride
-    __shared__ float sLoss[4];
 
     const uint32_t tid = threadIdx.x;
     const uint32_t q = blockIdx.x * 128 + tid;
@@ -912,24 +924,8 @@ __global__ void __launch_bounds__(128) k_nrcTrain(NrcLevels levels, const __half
             o[j] = __float2half(acc);
         }
     }
-    // loss + dL/dy (relative_l2_luminance.h:41-88)
-    float localLoss = 0.0f;
     __half* d = sD + (size_t)tid * kRowStride;
-    {
-        const uint32_t nTotal = numData * kOutputDims;
-        const float r = __half2float(o[0]), g = __half2float(o[1]), b = __half2float(o[2]);
-        const float luminance = 0.299f * r + 0.587f * g + 0.114f * b;
-        const float denom = luminance * luminance + 0.01f;
-        for (uint32_t k = 0; k < kPaddedOutput; ++k) {
-            float gr = 0.0f;
-            if (k < kOutputDims && valid) {
-                const float difference = __half2float(o[k]) - target[(size_t)q * kOutputDims + k];
-                localLoss += difference * difference / denom / nTotal;
-                gr = kLossScale * (2 * difference / denom) / nTotal;
-            }
-            d[k] = __float2half(gr);
-        }
-    }
+    const float localLoss = nrcRelativeL2Luminance(o, target + (size_t)q * kOutputDims, valid, numData, d);
     __syncthreads();
 
     // output layer: dW, then dL/d(hidden)
@@ -987,44 +983,11 @@ __global__ void __launch_bounds__(128) k_nrcTrain(NrcLevels levels, const __half
         __syncthreads();
     }
 
-    // hash-grid backward (kernel_grid_backward, grid.h:306-429): scatter the first 32 input gradients
-    if (kEnc == kEncHashGrid && valid) {
-        unsigned long long* gGrid = grads + numMatrixWeights;
-        const float* in = input + (size_t)q * kInputDims;
-        for (uint32_t l = 0; l < kLevels; ++l) {
-            const NrcLevel lv = levels.l[l];
-            const float g0 = __half2float(d[l * 2 + 0]), g1 = __half2float(d[l * 2 + 1]);
-            if (g0 == 0.0f && g1 == 0.0f)
-                continue;
-            float pos[3];
-            uint32_t posGrid[3];
-            for (uint32_t dd = 0; dd < 3; ++dd) {
-                pos[dd] = in[dd] * lv.scale + 0.5f;
-                const int tmp = (int)floorf(pos[dd]);
-                posGrid[dd] = (uint32_t)tmp;
-                pos[dd] -= (float)tmp;
-            }
-            const NrcCellIndexer indexer(lv, posGrid);
-#pragma unroll
-            for (uint32_t idx = 0; idx < 8; ++idx) {
-                float weight = 1;
-#pragma unroll
-                for (uint32_t dd = 0; dd < 3; ++dd)
-                    weight *= (idx & (1u << dd)) == 0 ? 1 - pos[dd] : pos[dd];
-                const uint32_t gi = lv.offset * 2 + indexer.corner(idx);
-                atomicAddFixed(gGrid + gi, weight * g0);
-                atomicAddFixed(gGrid + gi + 1, weight * g1);
-            }
-        }
-    }
-    // block loss
-    for (int off = 16; off > 0; off >>= 1)
-        localLoss += __shfl_xor_sync(0xFFFFFFFFu, localLoss, off);
-    if ((tid & 31) == 0)
-        sLoss[tid >> 5] = localLoss;
-    __syncthreads();
-    if (tid == 0)
-        atomicAdd(lossOut, sLoss[0] + sLoss[1] + sLoss[2] + sLoss[3]);
+    // the first 32 input gradients, to the hash grid
+    if (kEnc == kEncHashGrid && valid)
+        nrcGridBackward(levels, input + (size_t)q * kInputDims, [&](uint32_t k) { return __half2float(d[k]); },
+                        grads + numMatrixWeights);
+    nrcBlockLoss(localLoss, lossOut);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1050,24 +1013,6 @@ GFX_D __half tileHalf(const uint8_t* tile, uint32_t row, uint32_t k) {
     return *reinterpret_cast<const __half*>(tile + (k / 8) * (kTileRows * 16) + row * 16 + (k % 8) * 2);
 }
 
-__global__ void k_nrcPrepTrainWeights(const __half* __restrict__ w, uint32_t numHiddenLayers, __half* __restrict__ blobFwd,
-                                      __half* __restrict__ blobT) {
-    const uint32_t total = numHiddenLayers * kWidth * kWidth + kPaddedOutput * kWidth;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < total; i += gridDim.x * blockDim.x) {
-        uint32_t layer = i / (kWidth * kWidth), rem = i % (kWidth * kWidth), N = kWidth;
-        if (layer >= numHiddenLayers) {
-            layer = numHiddenLayers;
-            rem = i - numHiddenLayers * kWidth * kWidth;
-            N = kPaddedOutput;
-        }
-        const uint32_t j = rem / kWidth, in = rem % kWidth; // W_l[j][in]
-        // forward blob: B[n = j][k = in]
-        blobFwd[layer * kWidth * kWidth + (in / 8) * (N * 8) + j * 8 + (in % 8)] = w[i];
-        // transposed blob: B[n = in][k = j], 64 rows per K-chunk
-        blobT[layer * kWidth * kWidth + (j / 8) * (kWidth * 8) + in * 8 + (j % 8)] = w[i];
-    }
-}
-
 template <uint32_t kEnc> // as k_nrcTrain: the triangle wave skips layer 0's data gradient and the encoding backward
 __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __half* __restrict__ params, uint32_t numMatrixWeights,
                                                     uint32_t numHiddenLayers, const uint4* __restrict__ blobFwd,
@@ -1084,40 +1029,20 @@ __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __ha
     uint8_t* sDzT = sDz + kATileBytes;                     // dZ^T tile [64 x 128] (rows = neurons, K = samples)
     uint8_t* sActT = sDzT + kTTileBytes;                   // A_l^T tile [64 x 128]
     __shared__ __align__(8) uint64_t weightBar;
-    __shared__ float sLoss[4];
 
     const uint32_t tid = threadIdx.x;
-    const uint32_t warp = tid >> 5;
     const uint32_t q = blockIdx.x * 128 + tid;
     const bool valid = q < numData;
-    const __half* table = params + numMatrixWeights;
 
     if (tid == 0) {
         mbarInit(&weightBar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(smemU32(&weightBar)), "r"(2 * weightBytes) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     :: "r"(smemU32(sWf)), "l"(blobFwd), "r"(weightBytes), "r"(smemU32(&weightBar)) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                     :: "r"(smemU32(sWt)), "l"(blobT), "r"(weightBytes), "r"(smemU32(&weightBar)) : "memory");
+        mbarExpectTx(&weightBar, 2 * weightBytes);
+        bulkLoad(sWf, blobFwd, weightBytes, &weightBar);
+        bulkLoad(sWt, blobT, weightBytes, &weightBar);
     }
 
-    // encode this thread's sample into A_0
-    if (valid) {
-        nrcEncodeQuery<kEnc>(levels, table, input + (size_t)q * kInputDims, [&](uint32_t c, const __half* f) {
-            uint4 v;
-            v.x = (uint32_t)__half_as_ushort(f[0]) | ((uint32_t)__half_as_ushort(f[1]) << 16);
-            v.y = (uint32_t)__half_as_ushort(f[2]) | ((uint32_t)__half_as_ushort(f[3]) << 16);
-            v.z = (uint32_t)__half_as_ushort(f[4]) | ((uint32_t)__half_as_ushort(f[5]) << 16);
-            v.w = (uint32_t)__half_as_ushort(f[6]) | ((uint32_t)__half_as_ushort(f[7]) << 16);
-            *reinterpret_cast<uint4*>(sAct + c * (kTileRows * 16) + tid * 16) = v;
-        });
-    }
-    else {
-#pragma unroll
-        for (uint32_t c = 0; c < 8; ++c)
-            *reinterpret_cast<uint4*>(sAct + c * (kTileRows * 16) + tid * 16) = make_uint4(0, 0, 0, 0);
-    }
+    encodeTileRow<kEnc>(levels, params + numMatrixWeights, input, q, numData, sAct, tid); // this thread's sample into A_0
     fenceProxyAsync();
     __syncthreads();
     mbarWait(&weightBar, 0);
@@ -1134,47 +1059,19 @@ __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __ha
     {
         float acc[2][8];
         mlpLayer16(acc, smemU32(sAct + H * kATileBytes), kTileRows * 16, smemU32(sWf) + H * kWidth * kWidth * 2);
-#pragma unroll
-        for (uint32_t h = 0; h < 2; ++h)
-#pragma unroll
-            for (uint32_t i = 0; i < 2; ++i)
-#pragma unroll
-                for (uint32_t e = 0; e < 2; ++e) {
-                    const uint32_t r = h * 64 + fragRow(tid, i), c = fragCol(tid, 0) + e;
-                    if (c < kOutputDims)
-                        sOutF[r * 4 + c] = acc[h][2 * i + e];
-                }
+        forEachOutput(acc, tid, [&](uint32_t r, uint32_t c, float v) { sOutF[r * 4 + c] = v; });
         __syncthreads();
     }
 
-    // ---- loss + dL/dy (relative_l2_luminance.h:41-88) -> this sample's row of dZ_H, fp16 like tiny-cuda-nn's backward buffers
-    float localLoss = 0.0f;
+    // ---- loss + dL/dy -> this sample's row of dZ_H
+    float localLoss;
     {
         const __half o[3] = { __float2half(sOutF[tid * 4 + 0]), __float2half(sOutF[tid * 4 + 1]), __float2half(sOutF[tid * 4 + 2]) };
-        const uint32_t nTotal = numData * kOutputDims;
-        const float rr = __half2float(o[0]), gg = __half2float(o[1]), bb = __half2float(o[2]);
-        const float luminance = 0.299f * rr + 0.587f * gg + 0.114f * bb;
-        const float denom = luminance * luminance + 0.01f;
         __half d[kPaddedOutput];
+        localLoss = nrcRelativeL2Luminance(o, target + (size_t)q * kOutputDims, valid, numData, d);
 #pragma unroll
-        for (uint32_t k = 0; k < kPaddedOutput; ++k) {
-            float gr = 0.0f;
-            if (k < kOutputDims && valid) {
-                const float difference = __half2float(o[k]) - target[(size_t)q * kOutputDims + k];
-                localLoss += difference * difference / denom / nTotal;
-                gr = kLossScale * (2 * difference / denom) / nTotal;
-            }
-            d[k] = __float2half(gr);
-        }
-#pragma unroll
-        for (uint32_t c = 0; c < kPaddedOutput / 8; ++c) {
-            uint4 v;
-            v.x = (uint32_t)__half_as_ushort(d[c * 8 + 0]) | ((uint32_t)__half_as_ushort(d[c * 8 + 1]) << 16);
-            v.y = (uint32_t)__half_as_ushort(d[c * 8 + 2]) | ((uint32_t)__half_as_ushort(d[c * 8 + 3]) << 16);
-            v.z = (uint32_t)__half_as_ushort(d[c * 8 + 4]) | ((uint32_t)__half_as_ushort(d[c * 8 + 5]) << 16);
-            v.w = (uint32_t)__half_as_ushort(d[c * 8 + 6]) | ((uint32_t)__half_as_ushort(d[c * 8 + 7]) << 16);
-            *reinterpret_cast<uint4*>(sDz + c * (kTileRows * 16) + tid * 16) = v;
-        }
+        for (uint32_t c = 0; c < kPaddedOutput / 8; ++c)
+            *reinterpret_cast<uint4*>(sDz + c * (kTileRows * 16) + tid * 16) = packHalf8(d + 8 * c);
     }
     __syncthreads(); // every thread has read its output row before sDzT is overwritten
 
@@ -1257,44 +1154,11 @@ __global__ void __launch_bounds__(128) k_nrcTrainTc(NrcLevels levels, const __ha
         __syncthreads(); // dZ_{l-1} is complete
     }
 
-    // ---- hash-grid backward (kernel_grid_backward, grid.h:306-429): scatter the first 32 input gradients (this sample's
-    // row of the dZ tile)
-    if (kEnc == kEncHashGrid && valid) {
-        unsigned long long* gGrid = grads + numMatrixWeights;
-        const float* in = input + (size_t)q * kInputDims;
-        for (uint32_t l = 0; l < kLevels; ++l) {
-            const NrcLevel lv = levels.l[l];
-            const float g0 = __half2float(tileHalf(sDz, tid, l * 2 + 0)), g1 = __half2float(tileHalf(sDz, tid, l * 2 + 1));
-            if (g0 == 0.0f && g1 == 0.0f)
-                continue;
-            float pos[3];
-            uint32_t posGrid[3];
-            for (uint32_t dd = 0; dd < 3; ++dd) {
-                pos[dd] = in[dd] * lv.scale + 0.5f;
-                const int tmp = (int)floorf(pos[dd]);
-                posGrid[dd] = (uint32_t)tmp;
-                pos[dd] -= (float)tmp;
-            }
-            const NrcCellIndexer indexer(lv, posGrid);
-#pragma unroll
-            for (uint32_t idx = 0; idx < 8; ++idx) {
-                float weight = 1;
-#pragma unroll
-                for (uint32_t dd = 0; dd < 3; ++dd)
-                    weight *= (idx & (1u << dd)) == 0 ? 1 - pos[dd] : pos[dd];
-                const uint32_t gi = lv.offset * 2 + indexer.corner(idx);
-                atomicAddFixed(gGrid + gi, weight * g0);
-                atomicAddFixed(gGrid + gi + 1, weight * g1);
-            }
-        }
-    }
-    for (int off = 16; off > 0; off >>= 1)
-        localLoss += __shfl_xor_sync(0xFFFFFFFFu, localLoss, off);
-    if ((tid & 31) == 0)
-        sLoss[warp] = localLoss;
-    __syncthreads();
-    if (tid == 0)
-        atomicAdd(lossOut, sLoss[0] + sLoss[1] + sLoss[2] + sLoss[3]);
+    // ---- the first 32 input gradients (this sample's row of the dZ tile), to the hash grid
+    if (kEnc == kEncHashGrid && valid)
+        nrcGridBackward(levels, input + (size_t)q * kInputDims, [&](uint32_t k) { return __half2float(tileHalf(sDz, tid, k)); },
+                        grads + numMatrixWeights);
+    nrcBlockLoss(localLoss, lossOut);
 }
 
 // adam_step (adam.h:49-115) + ema_step_half_precision (ema.h:61-77); clears the gradient for the next step
@@ -1648,21 +1512,29 @@ static int nrcEnsureScratch(gfx_nrc* n, uint32_t numQueries) {
     return GFX_OK;
 }
 
-// pack + grid encode (the two kernels in front of k_nrcInferMlp); numData (or *numDataPtr) is a multiple of 128
-static int nrcGridEncodeLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, uint32_t numData, const uint32_t* numDataPtr,
-                               bool emaTable) {
+static uint32_t nrcSmCount() {
     int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    return (uint32_t)sms;
+}
+
+// pack + grid encode of the inference weights' hash grid (the two kernels in front of k_nrcInferMlp); numData (or *numDataPtr)
+// is a multiple of 128
+static int nrcGridEncodeLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, uint32_t numData, const uint32_t* numDataPtr) {
+    int rc = nrcEnsureScratch(n, numData);
+    if (rc != GFX_OK)
+        return rc;
+    const uint32_t sms = nrcSmCount();
     { GFX_TIMED(n->ctx, s, "nrc_pack_positions");
     k_nrcPackPositions<<<sms * 4, 256, 0, s>>>(inputData, n->positions, numData, numDataPtr); }
     n->ctx->launches++;
-    const uint32_t replicas = (uint32_t)sms / kLevels > 0 ? (uint32_t)sms / kLevels : 1u;
+    const uint32_t replicas = sms / kLevels > 0 ? sms / kLevels : 1u;
     const size_t smem = (size_t)(1u << kLog2HashmapSize) * 4;
     NRC_CUDA(n, cudaFuncSetAttribute(k_nrcGridEncode, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     { GFX_TIMED(n->ctx, s, "nrc_grid_encode");
-    k_nrcGridEncode<<<kLevels * replicas, kEncodeThreads, smem, s>>>(n->levels, (emaTable ? n->paramsEma : n->params) + n->numMatrixWeights,
-                                                                     n->positions, n->features, replicas, numData, numDataPtr); }
+    k_nrcGridEncode<<<kLevels * replicas, kEncodeThreads, smem, s>>>(n->levels, n->paramsEma + n->numMatrixWeights, n->positions,
+                                                                     n->features, replicas, numData, numDataPtr); }
     n->ctx->launches++;
     NRC_CUDA(n, cudaGetLastError());
     return GFX_OK;
@@ -1671,13 +1543,11 @@ static int nrcGridEncodeLaunch(gfx_nrc* n, cudaStream_t s, const float* inputDat
 static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, float* predictionData, uint32_t numData,
                           const uint32_t* numDataPtr) {
     if (n->ummaDirty) {
-        k_nrcPrepWeights<<<32, 256, 0, s>>>(n->paramsEma, n->numHiddenLayers, reinterpret_cast<__half*>(n->ummaWeights));
+        k_nrcPrepWeights<<<32, 256, 0, s>>>(n->paramsEma, n->numHiddenLayers, reinterpret_cast<__half*>(n->ummaWeights), nullptr);
         n->ctx->launches++;
         n->ummaDirty = false;
     }
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const uint32_t sms = nrcSmCount();
     const uint32_t numTiles = numData / kTileRows; // upper bound when numDataPtr is given
     // buffers the TMA bulk copies cannot take (not 16-byte aligned) go through the one-kernel form, which encodes by L2 gathers
     // inside the MLP kernel
@@ -1687,7 +1557,7 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
         const size_t smem = nrcInferFusedSmem(n->numMatrixWeights);
         auto kernel = hashGrid ? k_nrcInfer<kEncHashGrid> : k_nrcInfer<kEncTriangleWave>;
         NRC_CUDA(n, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const uint32_t grid = numTiles < (uint32_t)sms * 6 ? numTiles : (uint32_t)sms * 6;
+        const uint32_t grid = numTiles < sms * 6 ? numTiles : sms * 6;
         GFX_TIMED(n->ctx, s, "nrc_infer");
         kernel<<<grid, 128, smem, s>>>(n->levels, n->paramsEma + n->numMatrixWeights, n->ummaWeights, n->numHiddenLayers,
                                        inputData, predictionData, numData, numDataPtr);
@@ -1695,33 +1565,21 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
         NRC_CUDA(n, cudaGetLastError());
         return GFX_OK;
     }
-    if (!hashGrid) { // triangle wave: one persistent kernel, nothing in front of it
-        const size_t smem = nrcInferMlpSmem<kEncTriangleWave>(n->numMatrixWeights);
-        NRC_CUDA(n, cudaFuncSetAttribute(k_nrcInferMlp<kEncTriangleWave>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const uint32_t ctasPerSm = (uint32_t)(220 * 1024 / (smem + 1024));
-        const uint32_t maxGrid = (uint32_t)sms * (ctasPerSm ? ctasPerSm : 1u);
-        const uint32_t grid = numTiles < maxGrid ? numTiles : maxGrid;
-        GFX_TIMED(n->ctx, s, "nrc_infer");
-        k_nrcInferMlp<kEncTriangleWave><<<grid, 128, smem, s>>>(n->ummaWeights, n->numHiddenLayers, inputData, nullptr,
-                                                                predictionData, numData, numDataPtr);
-        n->ctx->launches++;
-        NRC_CUDA(n, cudaGetLastError());
-        return GFX_OK;
+    // the triangle wave has nothing in front of the persistent MLP kernel
+    if (hashGrid) {
+        const int rc = nrcGridEncodeLaunch(n, s, inputData, numData, numDataPtr);
+        if (rc != GFX_OK)
+            return rc;
     }
-    int rc = nrcEnsureScratch(n, numData);
-    if (rc != GFX_OK)
-        return rc;
-    rc = nrcGridEncodeLaunch(n, s, inputData, numData, numDataPtr, true);
-    if (rc != GFX_OK)
-        return rc;
-    const size_t smem = nrcInferMlpSmem<kEncHashGrid>(n->numMatrixWeights);
-    NRC_CUDA(n, cudaFuncSetAttribute(k_nrcInferMlp<kEncHashGrid>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const size_t smem = hashGrid ? nrcInferMlpSmem<kEncHashGrid>(n->numMatrixWeights) : nrcInferMlpSmem<kEncTriangleWave>(n->numMatrixWeights);
+    auto kernel = hashGrid ? k_nrcInferMlp<kEncHashGrid> : k_nrcInferMlp<kEncTriangleWave>;
+    NRC_CUDA(n, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const uint32_t ctasPerSm = (uint32_t)(220 * 1024 / (smem + 1024));
-    const uint32_t maxGrid = (uint32_t)sms * (ctasPerSm ? ctasPerSm : 1u);
+    const uint32_t maxGrid = sms * (ctasPerSm ? ctasPerSm : 1u);
     const uint32_t grid = numTiles < maxGrid ? numTiles : maxGrid;
     GFX_TIMED(n->ctx, s, "nrc_infer");
-    k_nrcInferMlp<kEncHashGrid><<<grid, 128, smem, s>>>(n->ummaWeights, n->numHiddenLayers, inputData, n->features, predictionData,
-                                                        numData, numDataPtr);
+    kernel<<<grid, 128, smem, s>>>(n->ummaWeights, n->numHiddenLayers, inputData, n->features, predictionData, numData,
+                                   numDataPtr);
     n->ctx->launches++;
     NRC_CUDA(n, cudaGetLastError());
     return GFX_OK;
@@ -1729,19 +1587,14 @@ static int nrcInferLaunch(gfx_nrc* n, cudaStream_t s, const float* inputData, fl
 
 // test hook (gfx_nrc_encode_debug): the encoded network input of numData queries, [numData][64] halves, through the split path
 static int nrcEncodeDebug(gfx_nrc* n, cudaStream_t s, const float* inputData, uint32_t numData, void* outHalf) {
-    if (n->positionEncoding == GFX_NRC_POSITION_ENCODING_TRIANGLE_WAVE) {
-        k_nrcTriWaveEncoding<<<(numData + 127) / 128, 128, 0, s>>>(inputData, numData, reinterpret_cast<__half*>(outHalf));
-        n->ctx->launches++;
-        NRC_CUDA(n, cudaGetLastError());
-        return GFX_OK;
+    const bool hashGrid = n->positionEncoding == GFX_NRC_POSITION_ENCODING_HASH_GRID;
+    if (hashGrid) {
+        const int rc = nrcGridEncodeLaunch(n, s, inputData, numData, nullptr);
+        if (rc != GFX_OK)
+            return rc;
     }
-    int rc = nrcEnsureScratch(n, numData);
-    if (rc != GFX_OK)
-        return rc;
-    rc = nrcGridEncodeLaunch(n, s, inputData, numData, nullptr, true);
-    if (rc != GFX_OK)
-        return rc;
-    k_nrcAssembleEncoding<<<(numData + 127) / 128, 128, 0, s>>>(inputData, n->features, numData, reinterpret_cast<__half*>(outHalf));
+    auto kernel = hashGrid ? k_nrcAssembleEncoding<kEncHashGrid> : k_nrcAssembleEncoding<kEncTriangleWave>;
+    kernel<<<(numData + 127) / 128, 128, 0, s>>>(inputData, n->features, numData, reinterpret_cast<__half*>(outHalf));
     n->ctx->launches++;
     NRC_CUDA(n, cudaGetLastError());
     return GFX_OK;
@@ -1839,18 +1692,16 @@ int gfx_nrc_train(gfx_nrc* n, void* stream, const float* inputData, const float*
         return GFX_OK;
     cudaStream_t s = (cudaStream_t)stream;
     NRC_CUDA(n, cudaMemsetAsync(n->loss, 0, 4, s));
-    // Fully-connected layers on wgmma (forward, data gradient and weight gradient); the CUDA-core kernel stays for deep
-    // networks whose activation tiles do not fit in shared memory and as the A/B switch GFX_NRC_TRAIN_CUDACORES=1.
-    const char* cudaCoresEnv = getenv("GFX_NRC_TRAIN_CUDACORES");
-    const bool forceCudaCores = cudaCoresEnv && cudaCoresEnv[0] == '1';
+    // Fully-connected layers on wgmma (forward, data gradient and weight gradient); deeper networks, whose activation tiles do
+    // not fit in shared memory, train on CUDA cores.
     const bool hashGrid = n->positionEncoding == GFX_NRC_POSITION_ENCODING_HASH_GRID;
-    if (n->numHiddenLayers <= kMaxTcTrainHiddenLayers && !forceCudaCores) {
+    if (n->numHiddenLayers <= kMaxTcTrainHiddenLayers) {
         const size_t smem = nrcTrainTcSmem(n->numMatrixWeights, n->numHiddenLayers);
         auto kernel = hashGrid ? k_nrcTrainTc<kEncHashGrid> : k_nrcTrainTc<kEncTriangleWave>;
         NRC_CUDA(n, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         { GFX_TIMED(n->ctx, s, "nrc_train_prep_weights");
-        k_nrcPrepTrainWeights<<<32, 256, 0, s>>>(n->params, n->numHiddenLayers, reinterpret_cast<__half*>(n->trainBlobFwd),
-                                                 reinterpret_cast<__half*>(n->trainBlobT)); }
+        k_nrcPrepWeights<<<32, 256, 0, s>>>(n->params, n->numHiddenLayers, reinterpret_cast<__half*>(n->trainBlobFwd),
+                                            reinterpret_cast<__half*>(n->trainBlobT)); }
         n->ctx->launches++;
         { GFX_TIMED(n->ctx, s, "nrc_train_fwd_bwd");
         kernel<<<numData / 128, 128, smem, s>>>(n->levels, n->params, n->numMatrixWeights, n->numHiddenLayers, n->trainBlobFwd,
