@@ -107,7 +107,7 @@ assert NODE_DTYPE.itemsize == 80 and TRI_DTYPE.itemsize == 48 and HIT_DTYPE.item
 
 # enums
 TRACE_CLOSEST, TRACE_ANY, TRACE_STATS = 0, 1, 2
-PT_BASELINE, PT_NRC, PT_REGIR, PT_NRC_VISUALIZE_PREDICTION, PT_SVGF = 0, 1, 2, 3, 4  # GfxPathTraceVariant
+PT_BASELINE, PT_NRC, PT_REGIR, PT_NRC_VISUALIZE_PREDICTION, PT_SVGF, PT_NRC_INDIRECT = 0, 1, 2, 3, 4, 5  # GfxPathTraceVariant
 NRC_READ_MASTER, NRC_READ_TRAINING, NRC_READ_INFERENCE, NRC_READ_GRADIENTS = 0, 1, 2, 3  # gfx_nrc_read
 NRC_POSITION_ENCODING_TRIANGLE_WAVE, NRC_POSITION_ENCODING_HASH_GRID = 0, 1  # gfx_nrc_create_with_encoding (PositionEncoding)
 (RESTIR_INITIAL_RIS, RESTIR_INITIAL_AND_TEMPORAL_BIASED, RESTIR_INITIAL_AND_TEMPORAL_UNBIASED,

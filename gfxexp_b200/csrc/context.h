@@ -155,6 +155,7 @@ struct FrameState {
         void* shardComm = nullptr;          // ncclComm_t of the ranks that share the frame
         int shardRank = 0, shardWorld = 1;
         uint32_t* shardCounts = nullptr;    // [0 .. world) gathered counts of this round, [64] this rank's count
+        bool lastTraceIndirect = false;     // the last NRC path-trace launch was GFX_PT_NRC_INDIRECT: gfx_nrc_accumulate adds
         bool created = false;
     } nrc;
     // rearchitected ReSTIR (restir_rearch.cu), allocated on first use
@@ -293,7 +294,7 @@ int launchSVGF(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int p
 int launchSVGFDebugVisualize(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int view, float motionVectorOffset,
                              float motionVectorScale, uint32_t numFilteringStages);
 int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, int variant);
-int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p);
+int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p, bool indirect); // GFX_PT_NRC[_INDIRECT]
 int launchNrcVisualizePrediction(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* p);
 void regirGrid(const GfxFrameParams* p, uint32_t dim[3], float origin[3], float cellSize[3]); // regir.cu
 int ensurePathTraceBuffers(gfx_ctx* ctx);

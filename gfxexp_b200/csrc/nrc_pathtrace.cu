@@ -268,8 +268,10 @@ GFX_D void emitRaysNrc(const DevScene &s, const DevPathState &ps, const DevNrc &
 
 // pathTrace_raygen_generic<true> up to the path extension loop (optix_pathtracing_kernels.cu:95-283).  BUMP:
 // GfxFrameParams::enableBumpMapping (a kernel of its own, so that the frames without it run the code they ran before it existed;
-// likewise k_nrcBounce and k_nrcVisualizeQueries)
-template <bool BUMP>
+// likewise k_nrcBounce and k_nrcVisualizeQueries).  INDIRECT: GFX_PT_NRC_INDIRECT, the same paths, draws and training records,
+// but the rendering radiance leaves out what ReSTIR DI estimates at the primary vertex - its emission, the environment seen
+// directly and its NEE (the light sample is still drawn and, on a training path, its shadow ray still traced for the target)
+template <bool BUMP, bool INDIRECT>
 __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, DevNrc n) {
     const uint32_t x = blockIdx.x * 8 + threadIdx.x;
     const uint32_t y = p.y0 + blockIdx.y * 8 + threadIdx.y;
@@ -301,7 +303,7 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrame
         float primaryPathSpread = 0.0f;
 
         const uint4 gb0 = f.gb0[p.bufferIndex][pix];
-        f3 radiance(0.001f, 0.001f, 0.001f);
+        f3 radiance(INDIRECT ? f3(0.0f) : f3(0.001f, 0.001f, 0.001f));
         if (gb0.x != 0xFFFFFFFFu) {
             flags |= NRC_F_PRIMARY_HIT;
             GBufferHit h;
@@ -322,10 +324,15 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrame
             const f3 vOutLocal = shadingFrame.toLocal(vOut);
 
             radiance = f3(0.0f);
-            if (vOutLocal.z > 0 && mat->hasEmittance)
+            if (!INDIRECT && vOutLocal.z > 0 && mat->hasEmittance)
                 radiance += alpha * f3(mat->emittance[0], mat->emittance[1], mat->emittance[2]) / kPi;
             const BSDF bsdf = setupBsdfAtHit(s, h.mesh, gb0.z, h.bcB, h.bcC);
-            shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, &radiance, &v);
+            f3 neeNotRendered(0.0f);
+            shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, INDIRECT ? &neeNotRendered : &radiance, &v);
+            if (INDIRECT) { // only a training path needs the visibility (its NEE target); the ray adds nothing to the radiance
+                v.wantShadow = v.wantShadow && isTrainingPath;
+                v.pending = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+            }
             f.rng[pix] = rng.state;
             ps.alphaPdf[pix] = make_float4(v.alpha.x, v.alpha.y, v.alpha.z, v.dirPDensity);
             n.pathB[pix] = make_float4(v.localThroughput.x, v.localThroughput.y, v.localThroughput.z, 0.0f);
@@ -336,7 +343,7 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrame
                 createRadianceQuery(p, positionInWorld, shadingFrame.normal, vOut, bsdf, n.stagedQuery + 14 * (size_t)linearTileIndex);
             }
         }
-        else if (s.env.enabled) { // :323-331: the environment seen directly; the miss program left (u, v) in the barycentrics
+        else if (!INDIRECT && s.env.enabled) { // :323-331: the environment seen directly; the miss program left (u, v) in the barycentrics
             radiance = s.env.powerCoeff * envFetch(s.env, decodeBarycentric((uint16_t)(gb0.w & 0xFFFFu)), decodeBarycentric((uint16_t)(gb0.w >> 16)));
         }
         ps.radiance[pix] = make_float4(radiance.x, radiance.y, radiance.z, 0.0f);
@@ -345,8 +352,10 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrame
     emitRaysNrc(s, ps, n, ps.counters, 0u, lane, pix, positionInWorld, v, alive, req);
 }
 
-// pathTrace_closestHit_generic<true> (:363-623) + the loop bookkeeping (:285-311) on the queue of live paths
-template <bool BUMP>
+// pathTrace_closestHit_generic<true> (:363-623) + the loop bookkeeping (:285-311) on the queue of live paths.  INDIRECT: at
+// pathLength 2 the implicit light terms (emitter hit, environment on a miss) only feed the training target: ReSTIR DI samples the
+// primary vertex's direct light by light sampling alone, so they have no MIS partner left in the rendering radiance
+template <bool BUMP, bool INDIRECT>
 __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, DevNrc n, uint32_t round) {
     const uint32_t curQueue = round & 1u, nextQueue = curQueue ^ 1u;
     const uint32_t* roundCounters = ps.counters + 4 * round;
@@ -387,7 +396,14 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
             do {
                 if (hit.y == 0xFFFFFFFFu) { // pathTrace_miss_generic (:625-672): implicit environment light, MIS
                     if (s.env.enabled) {
-                        const f3 directContImplicit = addEnvLightOnMiss(s, ps, curQueue, slot, pix, true);
+                        f3 directContImplicit;
+                        if (INDIRECT && round == 0) {
+                            const float4 r1 = ps.extRays[curQueue][2 * (size_t)slot + 1];
+                            directContImplicit = evaluateEnvLightOnMiss(s, f3(r1.x, r1.y, r1.z), ps.alphaPdf[pix].w, true);
+                        }
+                        else {
+                            directContImplicit = addEnvLightOnMiss(s, ps, curQueue, slot, pix, true);
+                        }
                         const uint32_t prevTrainDataIndex = isTrainingPath ? n.tilePrev[tile] : kInvalidVertexDataIndex;
                         if (isTrainingPath && prevTrainDataIndex != kInvalidVertexDataIndex) {
                             const float4 pb = n.pathB[pix];
@@ -430,7 +446,8 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
                 if (vOutLocal.z > 0 && mat->hasEmittance) {
                     const f3 emittance(mat->emittance[0], mat->emittance[1], mat->emittance[2]);
                     const f3 directContImplicit = emittance * implicitEmissionWeight(h.sp.hypAreaPDensity, dist2, vOutLocal.z, prevDirPDensity);
-                    radiance += alpha * directContImplicit;
+                    if (!(INDIRECT && round == 0))
+                        radiance += alpha * directContImplicit;
                     if (isTrainingPath && prevTrainDataIndex != kInvalidVertexDataIndex) {
                         const float4 pb = n.pathB[pix];
                         const f3 add = f3(pb.x, pb.y, pb.z) * directContImplicit;
@@ -679,7 +696,7 @@ struct NrcShadowWriter { // ShadowAccumulateWriter + the NEE target of the train
     }
 };
 
-int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params) {
+int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* params, bool indirect) {
     int rc = ensurePathTraceBuffers(ctx);
     if (rc != GFX_OK)
         return rc;
@@ -690,19 +707,20 @@ int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* 
     const DevFrameParams p = makeDevParams(ctx, params);
     // a strip of rows (tileOriginY / tileRows) is one rank's share of a frame sharded with gfx_nrc_shard: the training
     // vertices are numbered over the whole frame, so a strip without the other ranks would leave holes in the records
+    const std::string where = indirect ? "gfx_pathtrace_launch(GFX_PT_NRC_INDIRECT)" : "gfx_pathtrace_launch(GFX_PT_NRC)";
     const bool sharded = F.nrc.shardComm != nullptr && F.nrc.shardWorld > 1;
     if (!sharded && (p.y0 != 0 || p.y1 != F.H)) {
-        ctx->setError("gfx_pathtrace_launch(GFX_PT_NRC): strips need gfx_nrc_shard (the training records span the frame)");
+        ctx->setError(where + ": strips need gfx_nrc_shard (the training records span the frame)");
         return GFX_ERR_INVALID_ARGUMENT;
     }
     if (p.y0 >= p.y1) {
-        ctx->setError("gfx_pathtrace_launch(GFX_PT_NRC): empty strip");
+        ctx->setError(where + ": empty strip");
         return GFX_ERR_INVALID_ARGUMENT;
     }
     typedef int (*NcclAllGatherFn)(const void*, void*, size_t, int, void*, cudaStream_t);
     const NcclAllGatherFn allGather = sharded ? reinterpret_cast<NcclAllGatherFn>(ncclSymbol("ncclAllGather")) : nullptr;
     if (sharded && !allGather) {
-        ctx->setError("gfx_pathtrace_launch(GFX_PT_NRC): ncclAllGather not found (load NCCL in the host process)");
+        ctx->setError(where + ": ncclAllGather not found (load NCCL in the host process)");
         return GFX_ERR_UNSUPPORTED;
     }
     const DevScene s = ctx->devScene(params);
@@ -723,16 +741,28 @@ int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* 
         WavefrontLabels{ "nrc_first_hit", "nrc_trace_shadow", "nrc_trace_extension", "nrc_bounce", "nrc_finish" },
         NrcShadowWriter{ ps.shadowPixel, ps.shadowPending, n.shadowPending2, ps.radiance, n.stagedIndex, n.trainTarget[0] }, true,
         [&](dim3 grid, dim3 block) {
-            if (bump)
-                k_nrcFirstHit<true><<<grid, block, 0, stream>>>(s, f, p, ps, n);
+            if (indirect) {
+                if (bump)
+                    k_nrcFirstHit<true, true><<<grid, block, 0, stream>>>(s, f, p, ps, n);
+                else
+                    k_nrcFirstHit<false, true><<<grid, block, 0, stream>>>(s, f, p, ps, n);
+            }
+            else if (bump)
+                k_nrcFirstHit<true, false><<<grid, block, 0, stream>>>(s, f, p, ps, n);
             else
-                k_nrcFirstHit<false><<<grid, block, 0, stream>>>(s, f, p, ps, n);
+                k_nrcFirstHit<false, false><<<grid, block, 0, stream>>>(s, f, p, ps, n);
         },
         [&](uint32_t blocks, uint32_t round) {
-            if (bump)
-                k_nrcBounce<true><<<blocks, 64, 0, stream>>>(s, f, p, ps, n, round);
+            if (indirect) {
+                if (bump)
+                    k_nrcBounce<true, true><<<blocks, 64, 0, stream>>>(s, f, p, ps, n, round);
+                else
+                    k_nrcBounce<false, true><<<blocks, 64, 0, stream>>>(s, f, p, ps, n, round);
+            }
+            else if (bump)
+                k_nrcBounce<true, false><<<blocks, 64, 0, stream>>>(s, f, p, ps, n, round);
             else
-                k_nrcBounce<false><<<blocks, 64, 0, stream>>>(s, f, p, ps, n, round);
+                k_nrcBounce<false, false><<<blocks, 64, 0, stream>>>(s, f, p, ps, n, round);
         },
         [&] {
             GFX_TIMED(ctx, stream, "nrc_commit");
@@ -750,10 +780,11 @@ int launchPathTraceNrc(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* 
             const uint32_t firstPixel = p.y0 * F.W, endPixel = p.y1 * F.W;
             k_nrcFinish<<<blocks, 256, 0, stream>>>(f, ps, n, firstPixel, endPixel);
         });
+    F.nrc.lastTraceIndirect = indirect;
     if (rc != GFX_OK)
         return rc;
     if (commitError) {
-        ctx->setError("gfx_pathtrace_launch(GFX_PT_NRC): ncclAllGather of the training-vertex counts failed");
+        ctx->setError(where + ": ncclAllGather of the training-vertex counts failed");
         return GFX_ERR_CUDA;
     }
     return GFX_OK;
@@ -814,7 +845,9 @@ int launchNrcVisualizePrediction(gfx_ctx* ctx, cudaStream_t stream, const GfxFra
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// nrc_setup_kernels.cu:51-92
+// nrc_setup_kernels.cu:51-92.  ADD: after GFX_PT_NRC_INDIRECT the beauty already holds this frame's ReSTIR DI blend
+// B = (1 - w) B_prev + w D, and the indirect estimate I is added with the same weight, B + w I: the running mean of D + I
+template <bool ADD>
 __global__ void __launch_bounds__(256) k_nrcAccumulate(DevFrame f, DevFrameParams p, DevNrc n) {
     const uint32_t i = p.y0 * f.W + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.y1 * f.W)
@@ -834,6 +867,13 @@ __global__ void __launch_bounds__(256) k_nrcAccumulate(DevFrame f, DevFrameParam
     }
     const f3 indirectCont = alpha * radiance;
     const f3 contribution = directCont + indirectCont;
+    if (ADD) {
+        const float4 b = f.beauty[i];
+        const float curWeight = 1.0f / (1 + p.numAccumFrames);
+        const f3 colorResult = f3(b.x, b.y, b.z) + curWeight * contribution;
+        f.beauty[i] = make_float4(colorResult.x, colorResult.y, colorResult.z, 1.0f);
+        return;
+    }
     f3 prevColorResult(0.0f);
     if (p.numAccumFrames > 0) {
         const float4 b = f.beauty[i];
@@ -983,7 +1023,12 @@ int launchNrcPass(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* param
     static const char* const kPassLabel[3] = { "nrc_accumulate", "nrc_propagate_merge", "nrc_shuffle" };
     GFX_TIMED(ctx, stream, kPassLabel[pass < 0 || pass > 2 ? 0 : pass]);
     switch (pass) {
-    case 0: k_nrcAccumulate<<<((p.y1 - p.y0) * ctx->frame.W + 255) / 256, 256, 0, stream>>>(ctx->devFrame(), p, n); break;
+    case 0:
+        if (ctx->frame.nrc.lastTraceIndirect)
+            k_nrcAccumulate<true><<<((p.y1 - p.y0) * ctx->frame.W + 255) / 256, 256, 0, stream>>>(ctx->devFrame(), p, n);
+        else
+            k_nrcAccumulate<false><<<((p.y1 - p.y0) * ctx->frame.W + 255) / 256, 256, 0, stream>>>(ctx->devFrame(), p, n);
+        break;
     case 1:
         k_nrcPropagate<<<(n.numSuffixes + 127) / 128, 128, 0, stream>>>(p, n, numPixels);
         if (n.shardWorld > 1) {

@@ -343,8 +343,8 @@ int launchPathTrace(gfx_ctx* ctx, cudaStream_t stream, const GfxFrameParams* par
         if (rc != GFX_OK)
             return rc;
     }
-    if (variant == GFX_PT_NRC)
-        return launchPathTraceNrc(ctx, stream, params);
+    if (variant == GFX_PT_NRC || variant == GFX_PT_NRC_INDIRECT)
+        return launchPathTraceNrc(ctx, stream, params, variant == GFX_PT_NRC_INDIRECT);
     if (variant == GFX_PT_NRC_VISUALIZE_PREDICTION)
         return launchNrcVisualizePrediction(ctx, stream, params);
     if (variant == GFX_PT_SVGF) { // the SVGF app has no bump mapping

@@ -340,15 +340,18 @@ class StripDriver:
             ctx._check(ctx.lib.gfx_nrc_shard(ctx.h, self.comm.handle, self.rank, self.world), "gfx_nrc_shard")
 
     def render_restir_nrc_frame(self, frame_index: int, offsets, num_spatial_passes: int = 1, unbiased: bool = False,
-                                train: bool = True):
+                                train: bool = True, combined: bool = False):
         """ReSTIR DI passes (as render_frame) then the NRC frame of engine.Context.nrc_frame on the same G-buffer, both on this
         rank's rows; `offsets` are the two perFrameRng() draws (identical on all ranks).  One all-gather of the beauty strips
-        at the end."""
+        at the end.
+        combined=False: the NRC frame blends its full path-traced estimate over the ReSTIR DI image.  combined=True: one
+        estimator, ReSTIR DI's direct light at the primary vertex plus the light beyond it from abi.PT_NRC_INDIRECT, added to
+        the beauty by nrc_accumulate; the training records are those of combined=False."""
         ctx, p = self.backend.ctx, self.params
         self.render_frame(frame_index, num_spatial_passes, unbiased, composite=False)
         self._tile(self.y0, self.y1)
         ctx.nrc_preprocess(p, offsets[0], offsets[1], frame_index == 0)
-        ctx.pathtrace(p, abi.PT_NRC)
+        ctx.pathtrace(p, abi.PT_NRC_INDIRECT if combined else abi.PT_NRC)
         self.wait_training()  # the weights of the previous frame's training steps; its shuffled records may be overwritten
         if self.world > 1:
             ctx._check(ctx.lib.gfx_nrc_frame_infer_rows(ctx.h, self.net.h, None, self.y0, self.y1), "gfx_nrc_frame_infer_rows")

@@ -15,7 +15,9 @@
 //   -position-encoding: the NRC network's position encoding, as the reference app's command line takes it
 //   (neural_radiance_caching_main.cpp:458, 755-766); hash grid by default.  nrc_params.f16 must hold that network's
 //   gfx_nrc_num_params halves.
-//   renderer: restir | restir_unbiased | rearch | rearch_unbiased | pathtrace | regir | nrc | svgf
+//   renderer: restir | restir_unbiased | rearch | rearch_unbiased | pathtrace | regir | nrc | restir_nrc | restir_nrc_unbiased | svgf
+//   restir_nrc[_unbiased]: ReSTIR DI + NRC as one estimator - the restir[_unbiased] frame, then the nrc frame's launches on the same
+//   G-buffer with GFX_PT_NRC_INDIRECT, whose gfx_nrc_accumulate adds the light beyond the primary vertex to ReSTIR DI's image.
 //   svgf: the SVGF app's frame (svgf_main.cpp:1980-2172) with its defaults - its own path tracer with specular mollification,
 //   temporal accumulation, variance, 5 a-trous stages, background, albedo modulation + TAA; its output is the filtered image
 //   GFX_BUF_SVGF_FINAL of the last frame instead of the beauty buffer.
@@ -195,8 +197,9 @@ int main(int argc, char** argv) {
         check(gfx, gfx_rng_seed(gfx, 591842031321323413ull), "gfx_rng_seed");              // restir_di_main.cpp:1309-1321
         check(gfx, gfx_restir_setup_neighbor_table(gfx), "gfx_restir_setup_neighbor_table");
 
-        const bool unbiased = renderer == "restir_unbiased" || renderer == "rearch_unbiased";
-        if (renderer == "nrc") {
+        const bool restirNrc = renderer == "restir_nrc" || renderer == "restir_nrc_unbiased";
+        const bool unbiased = renderer == "restir_unbiased" || renderer == "rearch_unbiased" || renderer == "restir_nrc_unbiased";
+        if (renderer == "nrc" || restirNrc) {
             check(gfx, gfx_nrc_create_with_encoding(gfx, positionEncoding, 2, 1e-2f, &nrc),  // neuralRadianceCache.initialize
                   "gfx_nrc_create_with_encoding");
             if (nrcParamsPath) {
@@ -217,6 +220,19 @@ int main(int argc, char** argv) {
 
         GfxFrameParams fp = scene.defaults;
         fp.enableBumpMapping = bumpMapping ? 1u : 0u;
+        // the NRC frame after its G-buffer pass (neural_radiance_caching_main.cpp:2270-2368)
+        auto nrcFrame = [&](bool newSequence, int variant) {
+            const uint32_t offsetToSelectUnbiasedTile = perFrameRng();
+            const uint32_t offsetToSelectTrainingPath = perFrameRng();
+            check(gfx, gfx_nrc_preprocess(gfx, nullptr, &fp, offsetToSelectUnbiasedTile, offsetToSelectTrainingPath, newSequence),
+                  "preprocessNRC");
+            check(gfx, gfx_pathtrace_launch(gfx, nullptr, &fp, variant), "pathTraceNRC");
+            check(gfx, gfx_nrc_frame_infer(gfx, nrc, nullptr), "neuralRadianceCache.infer");
+            check(gfx, gfx_nrc_accumulate(gfx, nullptr, &fp), "accumulateInferredRadianceValues");
+            check(gfx, gfx_nrc_propagate(gfx, nullptr, &fp), "propagateRadianceValues");
+            check(gfx, gfx_nrc_shuffle(gfx, nullptr, &fp), "shuffleTrainingData");
+            check(gfx, gfx_nrc_frame_train(gfx, nrc, nullptr, nullptr), "neuralRadianceCache.train");
+        };
         uint32_t lastSpatialNeighborBaseIndex = 0, lastReservoirIndex = 1;                 // restir_di_main.cpp:1685-1686
         const uint32_t numSpatialReusePasses = 1;
         double totalMs = 0.0;
@@ -232,7 +248,7 @@ int main(int argc, char** argv) {
             fp.useUnbiasedEstimator = unbiased;
             check(gfx, gfx_light_dist_build(gfx, nullptr, bufferIndex), "gfx_light_dist_build");
 
-            if (renderer == "restir" || renderer == "restir_unbiased") {                   // restir_di_main.cpp:2352-2421
+            if (renderer == "restir" || renderer == "restir_unbiased" || restirNrc) {      // restir_di_main.cpp:2352-2421
                 uint32_t currentReservoirIndex = (lastReservoirIndex + 1) % 2;
                 fp.currentReservoirIndex = currentReservoirIndex;
                 fp.spatialNeighborBaseIndex = lastSpatialNeighborBaseIndex;
@@ -253,6 +269,8 @@ int main(int argc, char** argv) {
                 }
                 check(gfx, gfx_restir_launch(gfx, nullptr, &fp, GFX_RESTIR_SHADING), "shading");
                 lastReservoirIndex = currentReservoirIndex;
+                if (restirNrc)
+                    nrcFrame(newSequence, GFX_PT_NRC_INDIRECT);
             }
             else if (renderer == "rearch" || renderer == "rearch_unbiased") {              // restir_di_main.cpp:2423-2493
                 const uint32_t currentReservoirIndex = (lastReservoirIndex + 1) % 2;
@@ -281,16 +299,7 @@ int main(int argc, char** argv) {
             }
             else if (renderer == "nrc") {                                                  // neural_radiance_caching_main.cpp:2256-2368
                 check(gfx, gfx_gbuffer_launch(gfx, nullptr, &fp), "gfx_gbuffer_launch");
-                const uint32_t offsetToSelectUnbiasedTile = perFrameRng();
-                const uint32_t offsetToSelectTrainingPath = perFrameRng();
-                check(gfx, gfx_nrc_preprocess(gfx, nullptr, &fp, offsetToSelectUnbiasedTile, offsetToSelectTrainingPath, newSequence),
-                      "preprocessNRC");
-                check(gfx, gfx_pathtrace_launch(gfx, nullptr, &fp, GFX_PT_NRC), "pathTraceNRC");
-                check(gfx, gfx_nrc_frame_infer(gfx, nrc, nullptr), "neuralRadianceCache.infer");
-                check(gfx, gfx_nrc_accumulate(gfx, nullptr, &fp), "accumulateInferredRadianceValues");
-                check(gfx, gfx_nrc_propagate(gfx, nullptr, &fp), "propagateRadianceValues");
-                check(gfx, gfx_nrc_shuffle(gfx, nullptr, &fp), "shuffleTrainingData");
-                check(gfx, gfx_nrc_frame_train(gfx, nrc, nullptr, nullptr), "neuralRadianceCache.train");
+                nrcFrame(newSequence, GFX_PT_NRC);
             }
             else if (renderer == "svgf") {                                                 // svgf_main.cpp:1980-2172
                 constexpr uint32_t numFilteringStages = 5;

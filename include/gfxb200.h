@@ -319,7 +319,7 @@ typedef enum GfxPathTraceVariant {
                                                  * buffers (gfx_nrc_preprocess creates them), GFX_ERR_UNSUPPORTED on a context
                                                  * sharded with gfx_nrc_shard(world > 1).  The next NRC frame overwrites
                                                  * everything it writes. */
-    GFX_PT_SVGF = 4                             /* the SVGF app's path tracer (svgf/gpu_kernels/optix_pathtracing_kernels.cu:
+    GFX_PT_SVGF = 4,                            /* the SVGF app's path tracer (svgf/gpu_kernels/optix_pathtracing_kernels.cu:
                                                  * 130-513, svgf_main.cpp:2118-2126) up to its temporal accumulation, which is
                                                  * GFX_SVGF_TEMPORAL_ACCUMULATE: from the G-buffer params->bufferIndex it writes
                                                  * one sample of max(contribution, 0) per pixel to GFX_BUF_BEAUTY_ACCUM and the
@@ -328,6 +328,14 @@ typedef enum GfxPathTraceVariant {
                                                  * shading normal as its geometric normal and frame; no Russian roulette at path
                                                  * length 2; GFX_SVGF_MOLLIFY_SPECULAR in params->svgfFlags regularises the
                                                  * bounces' BSDFs.  Rows params->tileOriginY / tileRows. */
+    GFX_PT_NRC_INDIRECT = 5                     /* GFX_PT_NRC for a frame whose direct light at the primary vertex comes from
+                                                 * ReSTIR DI: the same paths, RNG draws, Russian roulette, cache termination,
+                                                 * training records and sharding rules, but the rendering radiance
+                                                 * (GFX_BUF_NRC_FRAME_CONTRIBUTION) leaves out the primary hit's emission, the
+                                                 * environment seen directly, the primary vertex's NEE (its shadow ray is traced
+                                                 * for training paths only) and, at path length 2, the implicit emitter and
+                                                 * environment terms; the training targets keep them.  The gfx_nrc_accumulate
+                                                 * that follows adds instead of blending (see there). */
 } GfxPathTraceVariant;
 
 /* SVGF entry points (svgf/svgf_main.cpp:2127-2172) */
@@ -741,6 +749,10 @@ int gfx_nrc_preprocess(gfx_ctx* ctx, void* stream, const GfxFrameParams* params,
 int gfx_nrc_frame_infer(gfx_ctx* ctx, gfx_nrc* nrc, void* stream);
 /* replaces kernelAccumulateInferredRadianceValues / kernelPropagateRadianceValues / kernelShuffleTrainingData
  * (:2320-2348; nrc_setup_kernels.cu:51-92, 94-138, 140-216) */
+/* gfx_nrc_accumulate after gfx_pathtrace_launch(GFX_PT_NRC_INDIRECT) (the context's last NRC path-trace launch) adds instead:
+ * beauty += w * (frame contribution + alpha * cache), w = 1 / (1 + params->numAccumFrames).  Precondition: this frame's ReSTIR DI
+ * shading pass has blended its direct light D into GFX_BUF_BEAUTY_ACCUM with the same numAccumFrames; the beauty is then the
+ * running mean of D + the NRC path tracer's light beyond the primary vertex (ReSTIR DI + NRC as one estimator). */
 int gfx_nrc_accumulate(gfx_ctx* ctx, void* stream, const GfxFrameParams* params);
 int gfx_nrc_propagate(gfx_ctx* ctx, void* stream, const GfxFrameParams* params);
 int gfx_nrc_shuffle(gfx_ctx* ctx, void* stream, const GfxFrameParams* params);
