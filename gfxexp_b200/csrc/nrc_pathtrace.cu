@@ -354,7 +354,11 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcFirstHit(DevScene s, DevFrame f, DevFrame
 
 // pathTrace_closestHit_generic<true> (:363-623) + the loop bookkeeping (:285-311) on the queue of live paths.  INDIRECT: at
 // pathLength 2 the implicit light terms (emitter hit, environment on a miss) only feed the training target: ReSTIR DI samples the
-// primary vertex's direct light by light sampling alone, so they have no MIS partner left in the rendering radiance
+// primary vertex's direct light by light sampling alone, so they have no MIS partner left in the rendering radiance.
+// Once a training path's rendering path has ended in the cache, its continuation feeds the training records only: the
+// cache at the terminal vertex already stands for all the light scattered there, so the NEE, emitter and environment
+// terms beyond it stay out of the rendering radiance (the reference adds them, optix_pathtracing_kernels.cu:549, :650,
+// and counts that light twice; DESIGN.md)
 template <bool BUMP, bool INDIRECT>
 __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFrameParams p, DevPathState ps, DevNrc n, uint32_t round) {
     const uint32_t curQueue = round & 1u, nextQueue = curQueue ^ 1u;
@@ -397,14 +401,14 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
                 if (hit.y == 0xFFFFFFFFu) { // pathTrace_miss_generic (:625-672): implicit environment light, MIS
                     if (s.env.enabled) {
                         f3 directContImplicit;
-                        if (INDIRECT && round == 0) {
+                        if ((INDIRECT && round == 0) || renderingPathEndsWithCache) {
                             const float4 r1 = ps.extRays[curQueue][2 * (size_t)slot + 1];
                             directContImplicit = evaluateEnvLightOnMiss(s, f3(r1.x, r1.y, r1.z), ps.alphaPdf[pix].w, true);
                         }
                         else {
                             directContImplicit = addEnvLightOnMiss(s, ps, curQueue, slot, pix, true);
                         }
-                        const uint32_t prevTrainDataIndex = isTrainingPath ? n.tilePrev[tile] : kInvalidVertexDataIndex;
+                        const uint32_t prevTrainDataIndex = isTrainingPath && n.tileSuffixEnded[tile] == 0 ? n.tilePrev[tile] : kInvalidVertexDataIndex;
                         if (isTrainingPath && prevTrainDataIndex != kInvalidVertexDataIndex) {
                             const float4 pb = n.pathB[pix];
                             const f3 addT = f3(pb.x, pb.y, pb.z) * directContImplicit;
@@ -423,8 +427,9 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
                 const float4 rad = ps.radiance[pix];
                 f3 radiance(rad.x, rad.y, rad.z);
                 PCG32RNG rng{ f.rng[pix] };
-                const uint32_t prevTrainDataIndex = isTrainingPath ? n.tilePrev[tile] : kInvalidVertexDataIndex;
-                bool trainingSuffixEndsWithCache = isTrainingPath ? n.tileSuffixEnded[tile] != 0 : false;
+                const bool trainingSuffixEndsWithCache = isTrainingPath ? n.tileSuffixEnded[tile] != 0 : false;
+                // a suffix ended by a full record buffer (k_nrcCommitScatter) still traces on: its later vertices feed no record
+                const uint32_t prevTrainDataIndex = isTrainingPath && !trainingSuffixEndsWithCache ? n.tilePrev[tile] : kInvalidVertexDataIndex;
 
                 HitVertex h;
                 setupHitVertex<BUMP>(s, hit, rayDir, &h);
@@ -446,7 +451,7 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
                 if (vOutLocal.z > 0 && mat->hasEmittance) {
                     const f3 emittance(mat->emittance[0], mat->emittance[1], mat->emittance[2]);
                     const f3 directContImplicit = emittance * implicitEmissionWeight(h.sp.hypAreaPDensity, dist2, vOutLocal.z, prevDirPDensity);
-                    if (!(INDIRECT && round == 0))
+                    if (!(INDIRECT && round == 0) && !renderingPathEndsWithCache)
                         radiance += alpha * directContImplicit;
                     if (isTrainingPath && prevTrainDataIndex != kInvalidVertexDataIndex) {
                         const float4 pb = n.pathB[pix];
@@ -520,7 +525,11 @@ __global__ void GFX_BOUNCE_BOUNDS k_nrcBounce(DevScene s, DevFrame f, DevFramePa
                     *vi = t;
                 }
 
-                shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha, &radiance, &v);
+                f3 neeNotRendered(0.0f);
+                shadeVertex(s, positionInWorld, vOutLocal, shadingFrame, bsdf, rng, alpha,
+                            renderingPathEndsWithCache ? &neeNotRendered : &radiance, &v);
+                if (renderingPathEndsWithCache) // the shadow ray still feeds the NEE target (NrcShadowWriter), not the radiance
+                    v.pending = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
                 ps.alphaPdf[pix] = make_float4(v.alpha.x, v.alpha.y, v.alpha.z, v.dirPDensity);
                 n.pathB[pix] = make_float4(v.localThroughput.x, v.localThroughput.y, v.localThroughput.z, 0.0f);
                 alive = true;

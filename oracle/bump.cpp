@@ -659,8 +659,9 @@ static void nrcExtendBump(orc_frame* f, orc_nrc_frame* n, const GfxFrameParams* 
     if (hit.primIndex == UINT32_MAX) { // pathTrace_miss_generic (:625-672)
         if (useEnvLight(s, p)) {
             const float3 directContImplicit = evaluateEnvLightOnMiss(s, p, st.rayDir, st.prevDirPDensity, true);
-            st.contribution += st.alpha * directContImplicit;
-            if (st.isTrainingPath && st.prevTrainDataIndex != kInvalidVertexDataIndex) {
+            if (!st.renderingPathEndsWithCache)
+                st.contribution += st.alpha * directContImplicit;
+            if (st.isTrainingPath && !st.trainingSuffixEndsWithCache && st.prevTrainDataIndex != kInvalidVertexDataIndex) {
                 float* tgt = &n->trainTarget[0][3 * (size_t)st.prevTrainDataIndex];
                 const float3 add = st.prevLocalThroughput * directContImplicit;
                 tgt[0] += add.x; tgt[1] += add.y; tgt[2] += add.z;
@@ -691,8 +692,9 @@ static void nrcExtendBump(orc_frame* f, orc_nrc_frame* n, const GfxFrameParams* 
         const float bsdfPDensity = st.prevDirPDensity;
         const float misWeight = pow2(bsdfPDensity) / (pow2(bsdfPDensity) + pow2(lightPDensity));
         const float3 directContImplicit = emittance * (misWeight / kPi);
-        st.contribution += st.alpha * directContImplicit;
-        if (st.isTrainingPath && st.prevTrainDataIndex != kInvalidVertexDataIndex) {
+        if (!st.renderingPathEndsWithCache)
+            st.contribution += st.alpha * directContImplicit;
+        if (st.isTrainingPath && !st.trainingSuffixEndsWithCache && st.prevTrainDataIndex != kInvalidVertexDataIndex) {
             float* tgt = &n->trainTarget[0][3 * (size_t)st.prevTrainDataIndex];
             const float3 add = st.prevLocalThroughput * directContImplicit;
             tgt[0] += add.x; tgt[1] += add.y; tgt[2] += add.z;
@@ -747,14 +749,15 @@ static void nrcExtendBump(orc_frame* f, orc_nrc_frame* n, const GfxFrameParams* 
     if (terminatedByRR)
         return;
     st.alpha *= recContinueProb;
-    if (st.isTrainingPath && st.prevTrainDataIndex != kInvalidVertexDataIndex) {
+    if (st.isTrainingPath && !st.trainingSuffixEndsWithCache && st.prevTrainDataIndex != kInvalidVertexDataIndex) {
         uint32_t* vi = &n->trainVertexInfo[4 * (size_t)st.prevTrainDataIndex];
         for (int c = 0; c < 3; ++c)
             vi[c] = f2u(u2f(vi[c]) * recContinueProb);
     }
 
     const float3 directContNEE = performNextEventEstimation(s, p, positionInWorld, vOutLocal, shadingFrame, bsdf, st.rng, counters);
-    st.contribution += st.alpha * directContNEE;
+    if (!st.renderingPathEndsWithCache)
+        st.contribution += st.alpha * directContNEE;
 
     float3 vInLocal;
     float dirPDensity;
